@@ -1,4 +1,4 @@
-/* nmsm — C ABI of the B200-native scalar-multiplication / MSM engine.
+/* nmsm — C ABI of the H100-native (sm_90a) scalar-multiplication / MSM engine.
  *
  * This is the drop-in boundary for noble-curves' hot path (SURVEY §8b).  noble has no FFI of its
  * own; these entry points are what an N-API addon (see INTEGRATION.md) binds behind the reference's

@@ -1,4 +1,4 @@
-// libnmsm.so — C ABI (include/nmsm.h) over the sm_100a kernels in msm.cuh.
+// libnmsm.so — C ABI (include/nmsm.h) over the sm_90a kernels in msm.cuh.
 // The per-curve engines are instantiated in inst_*.cu (compiled in parallel); this file holds the
 // process-wide context, the Montgomery-multiplication microbenchmark and the extern "C" surface.
 // There is deliberately no CPU path: every entry point needs a CUDA device.
@@ -97,7 +97,7 @@ bool stage_init() {
   StageState& S = g_stage;
   if (S.ready) return S.threads > 0;
   S.ready = true;
-  int want = 4;  // measured on the B200 box (15 host threads), 96 MB of bn254 inputs: 4 threads 3.1 ms, 6 threads 3.6 ms, driver staging 8.5 ms
+  int want = 4;  // worker threads (at most half the host's)
   if (const char* e = getenv("NMSM_STAGE_THREADS")) want = atoi(e);  // 0 disables the staged path
   const int hw = (int)std::thread::hardware_concurrency();
   if (hw > 0 && want > hw / 2) want = hw / 2;

@@ -95,7 +95,7 @@ static constexpr int NUM_SLOTS = NMSM_SLOTS;  // include/nmsm.h
 struct Context {
   bool ready = false;
   int device = -1;
-  int sm_count = 148;
+  int sm_count = 132;  // H100 SXM; nmsm_init reads the device's count
   Slot slot[NUM_SLOTS];
   int cur = 0;  // slot used by the call in progress (set by the C-ABI wrapper under the mutex)
   Buf ed_scratch;
@@ -114,8 +114,8 @@ struct Context {
 
 // H2D copy of a caller's host array, ordered before later work on `stream`.  Pinned (cudaHostAlloc / cudaHostRegister /
 // nmsm_host_alloc) sources go out as one cudaMemcpyAsync.  Large PAGEABLE sources — what a JS typed array or a Python
-// bytes object is — would be staged by the driver on ONE thread at ~12 GB/s (measured: 100 MB of bn254 points and
-// scalars 8.6 ms, twice the MSM itself); instead a few worker threads copy chunks into a ring of pinned staging buffers
+// bytes object is — would be staged by the driver on ONE thread, well below the pinned PCIe rate; instead a few worker
+// threads copy chunks into a ring of pinned staging buffers
 // and issue the chunk DMAs themselves, which keeps PCIe near its pinned rate.  capi.cu.
 int h2d_any(void* dst, const void* src, size_t bytes, cudaStream_t stream);
 void h2d_release();

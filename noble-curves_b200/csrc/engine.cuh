@@ -51,11 +51,10 @@ static int reduce2_r(uint64_t chunks) {
 
 static constexpr int SHARD_MIN_C = 8;  // sharded MSMs: at most ceil(257 / 8) = 33 windows (MAX_WINDOWS), one group each
 
-// How many window groups to pipeline.  Measured on B200 (2^20 BLS12-381 G1 terms, profiles/r02_trace_window_groups.txt):
-// overlapping the bucket reduction and Horner chains of finished groups with the accumulation of the rest does NOT
-// shorten one MSM — the latency-bound tail kernels share every SM sub-partition with 4 accumulate warps and run 3-5x
-// slower, the accumulation loses the pipe time they take (5.9 -> 6.6 ms), and the last group's tail stays on the
-// critical path: 8.36 ms with 8 groups vs 8.38 ms with one.  So one group is the default; nmsm_set_window_groups keeps
+// How many window groups to pipeline.  Overlapping the bucket reduction and Horner chains of finished groups with the
+// accumulation of the rest does not shorten one MSM: the latency-bound tail kernels share every SM sub-partition with
+// 4 accumulate warps and run several times slower, the accumulation loses the pipe time they take, and the last group's
+// tail stays on the critical path.  So one group is the default; nmsm_set_window_groups keeps
 // the pipelined form available, and sharded MSMs use one group per window because that is what lets a window's bucket
 // exchange overlap the accumulation of the next windows.
 static int choose_groups(const MsmPlan& plan, uint64_t max_entries) {
@@ -105,7 +104,7 @@ static int stage_host_inputs(Slot& C, const void* pts, const void* scalars, uint
 //                 k_horner_step with the window's weight 2^(c w)                                          -> ev_tail[w]
 //   comm stream   ncclAllGather of every rank's weighted window sums (+ its validation words); k_combine folds them.
 // With nmsm_set_window_groups(> 1): one group per window, top window first, the exchange of window w overlapping the
-// accumulation of windows w-1..0 (measured slower on B200 at 2, 4 and 8 GPUs: DESIGN.md §6).
+// accumulation of windows w-1..0 (slower than the bulk form for the reason given at choose_groups: DESIGN.md §6).
 static int submit_msm(const uint32_t* d_pts, const uint32_t* d_scalars, uint64_t n, uint32_t* d_out_acc,
                       const uint32_t* d_prepared, int table_c = 0, uint64_t table_points = 0,
                       const ShardArgs* shard = nullptr) {
@@ -187,8 +186,7 @@ static int submit_msm(const uint32_t* d_pts, const uint32_t* d_scalars, uint64_t
   cudaStream_t st = C.stream;
   const uint32_t n32 = (uint32_t)n;
   // sharded: one group per window (the exchange of window w overlaps the accumulation of the rest) or, the default, ONE
-  // group (bulk: one accumulate launch at full efficiency, one exchange step for all windows).  Measured on 2 B200,
-  // 2^20 terms in total: see profiles/r02_trace_sharded_*.txt
+  // group (bulk: one accumulate launch at full efficiency, one exchange step for all windows).
   int NG = choose_groups(plan, max_entries);
   if (shard) {
     NG = g_ctx.forced_groups ? (g_ctx.forced_groups >= plan.W ? plan.W : g_ctx.forced_groups) : 1;
@@ -848,9 +846,8 @@ static int run_mul_batch(const uint8_t* pts, const uint8_t* scalars, uint64_t n,
   CK(cudaMemcpyAsync(C.in_scalars.p, scalars, n * SCALAR_WORDS * 4, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(d_err, 0xff, 8, st));
   EV(0);
-  // one item per quad of lanes while that leaves the multiply pipe under-subscribed (<= 1.5 warps per sub-partition).
-  // Measured on B200 (profiles/r02_sweep_mul_batch.jsonl), kernel ms quad / serial: secp256k1 x 1024 0.81 / 1.19,
-  // x 8192 0.97 / 1.19; BLS12-381 G1 x 1024 2.13 / 3.45, x 16384 5.02 / 3.49 (serial wins once the pipe is full)
+  // one item per quad of lanes while that leaves the multiply pipe under-subscribed (<= 1.5 warps per sub-partition);
+  // one item per thread wins once the pipe is full
   uint64_t quad_max = (uint64_t)g_ctx.sm_count * 4 * 12;
   if (const char* e = getenv("NMSM_MUL_QUAD_MAX")) quad_max = strtoull(e, nullptr, 10);  // tuning experiments
   if (n <= quad_max)

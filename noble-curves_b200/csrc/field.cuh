@@ -400,7 +400,7 @@ NMSM_HD Fp<C> dbl(const Fp<C>& a) {
 
 // Modular inverse by a binary extended GCD on the limbs (modular.ts:980 `inv` -> :159-182; the reference runs extended
 // Euclid on BigInt): ~2*BITS shift/subtract steps.  Since round 2 this is only the FALLBACK of nmsm::inv
-// (inv_divsteps.cuh, batched division steps: 35 us instead of 217 us for a lone warp on B200, 381-bit field).
+// (inv_divsteps.cuh, batched division steps, several times faster for a lone warp).
 // Input and output in Montgomery form; 0 maps to 0.
 template <class C>
 NMSM_HD Fp<C> inv_xgcd(const Fp<C>& a) {

@@ -1,7 +1,7 @@
 // nmsm::inv — the field inversion every kernel uses (to-affine of results, warp_batch_inverse, table building, decoders).
 // Verified on the host against pow(x, -1, p) for all four base fields (tests/test_hostemu_parity.py::test_divsteps_inverse)
-// and on the GPU through every bit-exact point result.  Measured on B200 (tools/gpu/micro/tail_ops.cu, one warp, 381-bit
-// field): 35 us per inversion against 217 us for the binary extended GCD it replaced (field.cuh inv_xgcd, kept as fallback).
+// and on the GPU through every bit-exact point result.  It replaced the binary extended GCD (field.cuh inv_xgcd, kept as
+// fallback), which takes several times longer for a lone warp (tools/gpu/micro/tail_ops.cu times both).
 //
 // Modular inversion by batched division steps (Bernstein–Yang "safegcd" in its half-delta form): the state
 // (f, g) = (p, x) is advanced 30 division steps at a time from the low 30 bits alone, the 2x2 transition matrix

@@ -1,4 +1,4 @@
-// CUDA kernels (sm_100a) of the bucket-method multi-scalar multiplication and the batched scalar
+// CUDA kernels (sm_90a) of the bucket-method multi-scalar multiplication and the batched scalar
 // multiplication.  Thread bodies live in msm_body.cuh; this file is the launch geometry.
 //
 // Replaces /root/reference/src/abstract/curve.ts:863-905 `pippenger(c, points, scalars)`:
@@ -154,11 +154,10 @@ __device__ __noinline__ F warp_batch_inverse(const F& z) {
 
 // NMSM_PAIRED=1 builds k_accumulate with paired accumulation (msm_body.cuh accumulate_pairs_pass1/2: same-bucket
 // neighbours added in affine with one warp-shared inversion, 16 instead of 20 multiplications per two entries).  It is
-// bit-exact (hostemu + all GPU parity tests) and executes 20 % fewer multiplications, but on B200 it is SLOWER than the
-// plain loop — 2^20 BLS12-381 G1 terms: 7.09 ms (4 blocks/SM, 704 B of spills) / 6.78 ms (3 blocks/SM) against 6.04 ms —
-// because one 35 us inversion plus 12 scan multiplications per warp amortise over only ~28 pairs per lane, pass 1 is a
-// chain of dependent gathers with one multiplication each, and the extra live state spills.  Kept as a build option
-// (profiles/r02_ab_paired_accumulate.txt); the default is the plain mixed-addition loop.
+// bit-exact (hostemu + all GPU parity tests) and executes 20 % fewer multiplications, but it was slower than the plain
+// loop: one inversion plus 12 scan multiplications per warp amortise over only ~28 pairs per lane, pass 1 is a chain of
+// dependent gathers with one multiplication each, and the extra live state spills.  Kept as a build option; the default
+// is the plain mixed-addition loop.
 #ifndef NMSM_PAIRED
 #define NMSM_PAIRED 0
 #endif
@@ -169,7 +168,7 @@ __device__ __noinline__ F warp_batch_inverse(const F& z) {
 #define NMSM_ACC_WIDE_BYTES 257  // accumulators from this size on take the WIDE occupancy
 #endif
 #ifndef NMSM_ACC_MINBLOCKS
-#define NMSM_ACC_MINBLOCKS 4  // measured on B200 (BLS12-381 G1): 1 -> 6.41 ms, 3 -> 6.02 ms, 4 -> 5.91 ms per 2^20-term MSM
+#define NMSM_ACC_MINBLOCKS 4  // 4 x 128 threads per SM: <= 128 registers per thread of the 64 K-register file
 #endif
 template <class Cv>
 __global__ void __launch_bounds__(128, (sizeof(typename Cv::G::Acc) >= NMSM_ACC_WIDE_BYTES ? NMSM_ACC_MINBLOCKS_WIDE : NMSM_ACC_MINBLOCKS))

@@ -46,9 +46,8 @@ struct MsmPlan {
                     // two windows and the windows can be accumulated and reduced as independent launches
 };
 // Entries per accumulate thread: whole waves of the grid (4 blocks of 128 threads per SM) with at most 64 entries per
-// thread.  Longer segments mean fewer bucket partials for k_reduce1 to stitch (measured on B200, 2^20 BLS12-381 G1 terms:
-// L = 32 -> 56 takes reduce1 from 0.88 to 0.65 ms, the whole MSM from 8.40 to 8.28 ms), and sizing them to fill the last
-// wave keeps k_accumulate's tail short.
+// thread.  Longer segments mean fewer bucket partials for k_reduce1 to stitch, and sizing them to fill the last wave
+// keeps k_accumulate's tail short.
 NMSM_HD int plan_seg_len(double entries, int sm_count) {
   const double wave = (double)sm_count * 4.0 * 128.0;  // threads of one full wave
   const double waves = ceil(entries / (64.0 * wave));
@@ -74,8 +73,8 @@ template <class Cv>
 constexpr int split_of() { return Cv::GLV_KIND == 3 ? 4 : (Cv::GLV ? 2 : 1); }
 
 // ---------------------------------------------------------------------------------------------
-// plan selection: pick the window size c that minimises a TIME model of the pipeline, with constants
-// measured on B200 for BLS12-381 G1 (profiles/) and scaled by field size / formula cost for the others:
+// plan selection: pick the window size c that minimises a TIME model of the pipeline.  The constants are for
+// BLS12-381 G1, scaled by field size / formula cost for the others; only their ratios steer the choice of c:
 //   accumulate   entries * 0.352 ns            (k_accumulate at ~88 % of the multiply-pipe bound)
 //   reduce1      max( buckets * (1 + parts) adds at 0.93 ns each  [throughput],
 //                     K * (1 + parts_top) dependent adds at ~30 us each  [one thread's chain] )
@@ -132,11 +131,9 @@ inline MsmPlan make_plan(uint64_t n, int forced_c, int sm_count, uint64_t n_loca
   const double terms_local = n_local ? (double)n_local * split_of<Cv>() : terms;
   p.L = seg_len(terms_local * p.W);
   // reduce chunk: the first reduction level is a latency chain of 2K additions per chunk, and wants ~2 warps per SM
-  // sub-partition (~1100 warps on 148 SMs).  8 buckets per thread does that for the 262144 buckets of a c = 16, 8-window
+  // sub-partition (~1000 warps on 132 SMs).  8 buckets per thread does that for the 262144 buckets of a c = 16, 8-window
   // plan; plans with fewer buckets take 4, and at <= 65536 buckets 2 with one chunk per QUAD of lanes (reduce1_quad_form).
-  // Measured on B200, profiles/r02_sweep_tail.jsonl: secp256k1 2^16 (40960 buckets) 1.45 -> 1.02 ms (K = 4) -> 0.97 ms
-  // (K = 2), 2^20 5.63 -> 5.32 ms; BLS12-381 G2 2^18 (131072 buckets) 8.76 -> 8.68 ms; at 262144 buckets K = 4 loses
-  // (BLS12-381 G1 2^20: 8.10 -> 8.28 ms) and so does K = 2 on ed25519's 278528 (1.26 -> 1.35 ms).
+  // At 262144 buckets and more, the shorter chunks lose (too few additions per thread to hide the chain).
   const uint64_t nbuckets = (uint64_t)p.W * (uint64_t)p.B;
   int Kc = nbuckets <= 65536u ? 2 : (nbuckets <= 131072u ? 4 : K);
 #if !defined(__CUDA_ARCH__)

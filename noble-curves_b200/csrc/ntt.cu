@@ -12,8 +12,8 @@
 //   natural in,  brp out     : DIF passes                                               (fft.ts:550)
 //   brp in,      natural out : DIT passes                                               (fft.ts:549)
 //   brp in,      brp out     : permute, DIF passes                                      (fft.ts:544-548)
-// Bound (ncu, profiles/): the integer multiply pipe — one 256-bit Montgomery multiplication per butterfly; the
-// fmaheavy pipe is ~62 % active in k_ntt_pass while DRAM throughput stays below 5 % of peak.
+// Bound: the integer multiply pipe — one 256-bit Montgomery multiplication per butterfly against 64 bytes of tile traffic,
+// most of it in shared memory (64 KB per block: two blocks fit in an H100 SM's 228 KB).
 #include "context.h"
 #include "field.cuh"
 #include "inv_divsteps.cuh"

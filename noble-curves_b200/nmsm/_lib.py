@@ -14,7 +14,7 @@ import threading
 # do not alias (takes effect if the CUDA context has not been created yet; never overrides an explicit setting).
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 # The sharded MSM moves one 6 MB bucket array per window and peer with ncclSend/ncclRecv; NCCL's default of 1-2 channels
-# (CTAs) per peer caps such a transfer near 25 GB/s on NVLink (measured: 0.27 ms per window).  More point-to-point channels
+# (CTAs) per peer caps such a transfer far below the NVLink rate.  More point-to-point channels
 # = more CTAs copying in parallel.  NCCL caches these parameters at its first communicator, so they must be in the
 # environment before torch.distributed / the library create one; explicit user settings win.
 os.environ.setdefault("NCCL_MIN_P2P_NCHANNELS", "16")

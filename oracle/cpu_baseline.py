@@ -10,6 +10,7 @@ from __future__ import annotations
 import ctypes
 import os
 import subprocess
+import tempfile
 import time
 
 from . import noble_ref as R
@@ -21,10 +22,18 @@ _lib = None
 
 
 def build(force: bool = False) -> str:
-    os.makedirs(os.path.dirname(_SO), exist_ok=True)
-    if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(_SRC):
-        subprocess.check_call(["gcc", "-O3", "-march=native", "-shared", "-fPIC", "-pthread", _SRC, "-o", _SO])
-    return _SO
+    if not force and os.path.exists(_SO) and os.path.getmtime(_SO) >= os.path.getmtime(_SRC):
+        return _SO
+    so = _SO
+    try:
+        os.makedirs(os.path.dirname(so), exist_ok=True)
+        writable = os.access(os.path.dirname(so), os.W_OK)
+    except OSError:
+        writable = False
+    if not writable:  # read-only tree (e.g. bench.py after build()): compile into a temporary directory instead
+        so = os.path.join(tempfile.mkdtemp(prefix="nmsm_ref_msm_"), "libref_msm.so")
+    subprocess.check_call(["gcc", "-O3", "-march=native", "-shared", "-fPIC", "-pthread", _SRC, "-o", so])
+    return so
 
 
 def load():

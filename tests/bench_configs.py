@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
-"""Measure every BASELINE.json config on one B200 (parity-checked, CUDA-event kernel times where the MSM
+"""Measure every BASELINE.json config on one H100 (parity-checked, CUDA-event kernel times where the MSM
 pipeline is used).  The headline (configs[1]/metric at 2^20) is bench.py; this writes the companion table.
 
-    python tests/bench_configs.py > profiles/r01_configs.jsonl
+    python tests/bench_configs.py
 
 configs (BASELINE.json):
   0  secp256k1 Point.multiply batch of 1024 random scalars      (reference: CPU bigint; here also the GPU batch)
@@ -204,9 +204,9 @@ def ntt_config(tag, field, logn, reps=5):
     # algorithmic HBM bytes: ingest (r+w) + passes x (r+w) + emit (r+w) + copy back (r+w), 32 B elements
     alg_bytes = (passes + 3) * 2 * n * 32
     try:
-        peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", 6650.0)
+        peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", 3350.0)
     except Exception:
-        peak = 6650.0
+        peak = 3350.0  # H100 SXM data sheet
     return {"config": tag, "what": "NTT over Fr(%s), 2^%d elements, device-resident (generator 7)" % (field, logn), "n": n,
             "direct_ms": t, "inverse_ms": min(inv), "direct_brp_out_ms": min(brp), "root_table_ms": t_roots,
             "elements_per_s": n / (t * 1e-3), "butterflies_per_s": (n // 2) * logn / (t * 1e-3),

@@ -18,6 +18,9 @@
 
 using namespace nmsm;
 
+// plans are made for the SM count of the target GPU (H100 SXM: 132 SMs), as nmsm_init does from the device
+static constexpr int EMU_SM_COUNT = 132;
+
 // what k_accumulate runs per thread.  g_paired = 0 (the default build, NMSM_PAIRED=0): the plain mixed-addition loop;
 // g_paired = 1: the paired accumulation of the NMSM_PAIRED=1 build for the short-Weierstrass curves (the warp-shared
 // inversion of the kernel becomes a plain inversion of this thread's product) — both are parity-tested.
@@ -47,7 +50,7 @@ static int emu_msm_t(const uint32_t* pts, const uint32_t* scalars, uint32_t n, i
                      int groups = 1) {
   using G = typename Cv::G;
   // table_c != 0: fixed-base table route (nmsm_points_precompute + nmsm_msm_points)
-  MsmPlan plan = table_c ? make_table_plan<Cv>(n, canonical_table_bits<Cv>(table_c), 148) : make_plan<Cv>(n, forced_c, 148);
+  MsmPlan plan = table_c ? make_table_plan<Cv>(n, canonical_table_bits<Cv>(table_c), EMU_SM_COUNT) : make_plan<Cv>(n, forced_c, EMU_SM_COUNT);
   if (forced_L > 0) {
     plan.L = forced_L;
     plan.TPW = plan_tpw((uint64_t)n * split_of<Cv>() * (table_c ? plan.D : 1), plan.L);
@@ -141,7 +144,7 @@ template <class Cv>
 static int emu_shard_buckets_t(const uint32_t* pts, const uint32_t* scalars, uint32_t n_local, uint32_t n_total,
                                uint32_t* buckets_out, uint32_t* plan_out, uint32_t* err_out) {
   using G = typename Cv::G;
-  MsmPlan plan = make_plan<Cv>(n_total, 0, 148, n_local ? n_local : 1);
+  MsmPlan plan = make_plan<Cv>(n_total, 0, EMU_SM_COUNT, n_local ? n_local : 1);
   plan_out[0] = plan.c; plan_out[1] = plan.W; plan_out[2] = plan.B; plan_out[3] = G::ACC_WORDS;
   if (!buckets_out) return 0;  // plan query
   const size_t terms = (size_t)(n_local ? n_local : 1) * split_of<Cv>();
@@ -179,7 +182,7 @@ static int emu_shard_buckets_t(const uint32_t* pts, const uint32_t* scalars, uin
 template <class Cv>
 static int emu_owner_window_t(uint32_t n_total, int w, uint32_t* own, const uint32_t* recv, int npeers, uint32_t* out_acc) {
   using G = typename Cv::G;
-  MsmPlan plan = make_plan<Cv>(n_total, 0, 148, 1);
+  MsmPlan plan = make_plan<Cv>(n_total, 0, EMU_SM_COUNT, 1);
   const size_t WB = (size_t)plan.B * G::ACC_WORDS;
   for (uint32_t b = 0; b < (uint32_t)plan.B; b++) bucket_fold_body<Cv>(b, own, recv, npeers, WB);
   // the kernels index buckets / chunks / window sums globally: stage the window at its global position
@@ -271,10 +274,10 @@ static int emu_torsion_t(const uint32_t* pts, uint32_t n, uint8_t* out_ok, uint3
 // plan introspection for tests: out = {c, W, B, L, K, chunks, D, wb, r, stride, auto_c}
 template <class Cv>
 static int emu_plan_t(uint32_t n, int table_c_req, uint32_t* out) {
-  MsmPlan p = table_c_req ? make_table_plan<Cv>(n, canonical_table_bits<Cv>(table_c_req), 148) : make_plan<Cv>(n, 0, 148);
+  MsmPlan p = table_c_req ? make_table_plan<Cv>(n, canonical_table_bits<Cv>(table_c_req), EMU_SM_COUNT) : make_plan<Cv>(n, 0, EMU_SM_COUNT);
   out[0] = p.c; out[1] = p.W; out[2] = p.B; out[3] = p.L; out[4] = p.K; out[5] = p.chunks; out[6] = p.D;
   out[7] = p.wb; out[8] = p.r; out[9] = p.stride;
-  out[10] = choose_table_bits<Cv>(n, 148, 64e9);
+  out[10] = choose_table_bits<Cv>(n, EMU_SM_COUNT, 64e9);
   out[11] = glv_bits<Cv>() + 1;
   return 0;
 }

@@ -3,7 +3,7 @@
 tests/hostemu compiles the *device* headers for the host with an emulated PTX carry flag and runs the
 per-thread kernel bodies in loops.  These tests compare that against the oracle bit-for-bit, mirroring
 the reference's MSM tests (test/point.test.ts:264-305,685-722,825-862; test/slow-curves.test.ts:185-252)
-and field tests (test/modular.test.ts).  The real parity tests (through libnmsm.so on a B200) are in
+and field tests (test/modular.test.ts).  The real parity tests (through libnmsm.so on an H100) are in
 test_gpu_parity.py.
 """
 import random

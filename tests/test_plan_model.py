@@ -1,5 +1,5 @@
 """Host-side plan selection (csrc/msm_body.cuh make_plan / make_table_plan / choose_table_bits), through the host
-emulation library: structural invariants the kernels rely on, and the choices the measurements in profiles/ back."""
+emulation library: structural invariants the kernels rely on, and the choices the time model makes at the BASELINE sizes."""
 import ctypes
 
 import numpy as np
@@ -32,7 +32,7 @@ def test_ordinary_plans(name):
     if name == "secp256k1":  # 130 half-scalar bits: c = 16 would leave a 2-bit top window (two giant buckets)
         assert big["c"] == 13 and big["W"] == 10
     elif name in ("bls12_381_G1", "bn254_G1", "bls12_381_G2", "bls12_381_G1_any", "bls12_381_G2_any"):
-        assert big["c"] == 16  # the measured configurations at the BASELINE sizes (profiles/)
+        assert big["c"] == 16
     else:
         assert 13 <= big["c"] <= 16
 
@@ -53,7 +53,7 @@ def test_table_plans_spread_the_digits_evenly(name):
 
 
 def test_table_window_choice_tracks_the_measurements():
-    assert plan("bls12_381_G1", 1 << 20)["auto_c"] == 19   # 7 digits: 7.55 ms vs 8.72 ms (r01_configs_fixed_base_v10)
-    assert plan("bls12_381_G1", 1 << 16)["auto_c"] == 16   # 1.59 ms at c = 16 vs 2.02 ms at c = 19
-    assert plan("bls12_381_G2", 1 << 18)["auto_c"] == 16   # 8.9 ms at c = 16 vs 9.2 ms at c = 19
+    assert plan("bls12_381_G1", 1 << 20)["auto_c"] == 19   # 7 digits
+    assert plan("bls12_381_G1", 1 << 16)["auto_c"] == 16
+    assert plan("bls12_381_G2", 1 << 18)["auto_c"] == 16
     assert plan("bn254_G1", 1 << 20)["auto_c"] == 19

@@ -1,9 +1,9 @@
-// EXPERIMENT (not part of libnmsm.so; measured by tools/gpu/micro/tail_ops.cu, results in profiles/r02_micro_tail_ops.jsonl):
-// none of these beat mont_mul for a lone warp on B200 (1917 cycles): c64 2501, sos 2488, lat4 2360 cycles.
+// EXPERIMENT (not part of libnmsm.so; measured by tools/gpu/micro/tail_ops.cu): none of these beat mont_mul for a
+// lone warp.
 // Latency-oriented Montgomery multiplication variants (experiments for the single-warp tails: Horner, reduce2/3, folds).
 // mont_mul (field.cuh) is tuned for THROUGHPUT: two interleaved carry chains saturate the multiply pipe once >= 2 warps share
 // an SM sub-partition, but a lone warp pays the ~13-cycle carry-to-carry latency of IMAD.WIDE.X on every link
-// (measured: 1917 cycles per 381-bit multiplication, 6.4 cycles per IMAD).  The variants here expose more independent work.
+// The variants here expose more independent work.
 #pragma once
 #include "field.cuh"
 

@@ -1,5 +1,5 @@
 // Microbenchmark of the latency-bound primitives of the bucket-reduction / Horner tails (one warp, dependent chains).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 [-DNMSM_MUL_NOINLINE] -I noble-curves_b200/csrc
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 [-DNMSM_MUL_NOINLINE] -I noble-curves_b200/csrc
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdint.h>
@@ -80,16 +80,18 @@ void run(const char* name, int threads, int blocks, int iters) {
 }
 
 int main() {
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   // burst vs sustained: the same saturating multiply chain for 0.5 ms .. 60 ms
-  for (int it : {1024}) run<0>("mul_sat", 128, 148 * 4, it);
-  for (int it : {1024}) run<0>("mul_sat8", 128, 148 * 8, it);
-  for (int it : {256, 4096}) run<1>("sqr_sat", 128, 148 * 4, it);
-  run<11>("mul_c64_sat", 128, 148 * 4, 1024);
-  run<12>("mul_sos_sat", 128, 148 * 4, 1024);
-  run<13>("mul_lat4_sat", 128, 148 * 4, 1024);
+  for (int it : {1024}) run<0>("mul_sat", 128, sms * 4, it);
+  for (int it : {1024}) run<0>("mul_sat8", 128, sms * 8, it);
+  for (int it : {256, 4096}) run<1>("sqr_sat", 128, sms * 4, it);
+  run<11>("mul_c64_sat", 128, sms * 4, 1024);
+  run<12>("mul_sos_sat", 128, sms * 4, 1024);
+  run<13>("mul_lat4_sat", 128, sms * 4, 1024);
   const int IT = 512;
   for (int thr : {32}) {
-    for (int blocks : {1, 148 * 4}) {
+    for (int blocks : {1, sms * 4}) {
       run<0>("mul", thr, blocks, IT);
       run<10>("mul_inline", thr, blocks, IT);
       run<11>("mul_c64", thr, blocks, IT);

@@ -3,11 +3,12 @@
 # usage: tools/sass_hist.sh [round-tag]
 set -e
 tag=${1:-r02}
+mkdir -p profiles
 obj=noble-curves_b200/build/inst_bls381g1.o
 hist() { grep -oE "^\s+/\*[0-9a-f]+\*/\s+[A-Z0-9_.]+" | awk '{print $2}' | sort | uniq -c | sort -rn; }
 fn() { cuobjdump -sass "$obj" | awk -v pat="$1" '/Function : /{on=($0 ~ pat)} on'; }
 {
-  echo "# cuobjdump -sass $obj  (sm_100a, built by make -C noble-curves_b200)  -- k_accumulate<CurveBls381G1>"
+  echo "# cuobjdump -sass $obj  (sm_90a, built by make -C noble-curves_b200)  -- k_accumulate<CurveBls381G1>"
   echo "# whole function (kernel body + the out-of-line mul_call / sqr_call subroutines it carries)"
   fn "k_accumulateINS_13CurveBls381G1E" | hist
 } > profiles/${tag}_sass_k_accumulate_hist.txt
