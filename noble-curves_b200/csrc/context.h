@@ -98,7 +98,8 @@ struct Context {
   int sm_count = 132;  // H100 SXM; nmsm_init reads the device's count
   Slot slot[NUM_SLOTS];
   int cur = 0;  // slot used by the call in progress (set by the C-ABI wrapper under the mutex)
-  Buf ed_scratch;
+  Buf ed_scratch;              // signature-verification scratch (ed25519 and secp256k1 batches)
+  uint32_t* ecdsa_g_table = nullptr;  // fixed-point table of the secp256k1 generator, built by the first ECDSA verify
   Buf ntt_data, ntt_work, ntt_tmp, ntt_roots, ntt_aux;  // NTT staging / work / output / root table (ntt.cu)
   int ntt_key_field = -1, ntt_key_bits = -1;            // which root table ntt_roots holds
   uint64_t ntt_key_gen = 0;
@@ -203,6 +204,8 @@ struct EngineVTable {
 };
 int ed25519_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs, const uint64_t* msg_off,
                               uint64_t n, const uint8_t* z16, int* out_ok, long long* out_bad_index);
+int secp256k1_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off, const uint8_t* msgs,
+                                const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
 int decode_points_impl(int curve, const uint8_t* enc, uint64_t n, int flags, uint8_t* out_xy, uint8_t* out_status);
 int ntt_impl(int curve, void* values, int on_device, int log_n, uint64_t generator, int inverse, int brp_input,
              int brp_output);

@@ -1,0 +1,221 @@
+// secp256k1 ECDSA batch verification (SURVEY §8 row f5): one independent verdict per signature.
+//
+// The reference verifies one signature at a time: weierstrass.ts `ecdsa().verify` (noble-curves v2), with
+// format 'compact' and the options { prehash, lowS } (both default true for secp256k1):
+//   sig = r || s (64 B, big-endian); inside the reference's try (any failure = false):
+//   1 <= r, s < n;  P = Point.fromBytes(publicKey)  (33 B 02/03 + sqrt, or 65 B 04 + curve equation);
+//   lowS && s > n/2 -> false;  h = bits2int_modN(prehash ? sha256(msg) : msg)  (bits2int: > 8192 bytes throws);
+//   w = s^-1,  u1 = h w,  u2 = r w  (mod n);  R = u1 G + u2 P;  R == O -> false;  accept iff R.x mod n == r.
+// ECDSA has no batch equation (R's y is not in the signature), so the batch is data-parallel: per signature
+//   ecdsa_prepare_body  parse + range checks, lowS, key decode, SHA-256, bits2int mod n
+//   (kernel)            s^-1 through one warp-shared inversion per 32 signatures (msm.cuh warp_batch_inverse)
+//   ecdsa_store         u1, u2
+//   ecdsa_check_body    u1 G from the fixed-point table of G (table_mul_body), u2 Q (GLV scalar_mul_acc), complete
+//                       addition, and the x comparison in XYZZ coordinates without an inversion.
+// The two halves run as two kernels (inst_secp256k1.cu) so the SHA-256 / square-root state stays out of the scalar
+// multiplication's registers.  Bodies are host/device so tests/hostemu can run them.
+#pragma once
+#include "codec.cuh"
+#include "validate.cuh"
+
+namespace nmsm {
+
+using EcS = Fp<FnSecp256k1Mod>;
+static constexpr int ECDSA_PREHASH = 1;  // include/nmsm.h NMSM_ECDSA_PREHASH
+static constexpr int ECDSA_LOW_S = 2;    // include/nmsm.h NMSM_ECDSA_LOW_S
+static constexpr uint64_t ECDSA_MAX_RAW_MSG = 8192;  // bits2int: "input is too large" above this many bytes
+
+// ---- SHA-256 (FIPS 180-4) ---------------------------------------------------------------------
+NMSM_HD uint32_t sha256_k(int i) {
+  constexpr uint32_t K[64] = {
+      0x428a2f98u, 0x71374491u, 0xb5c0fbcfu, 0xe9b5dba5u, 0x3956c25bu, 0x59f111f1u, 0x923f82a4u, 0xab1c5ed5u,
+      0xd807aa98u, 0x12835b01u, 0x243185beu, 0x550c7dc3u, 0x72be5d74u, 0x80deb1feu, 0x9bdc06a7u, 0xc19bf174u,
+      0xe49b69c1u, 0xefbe4786u, 0x0fc19dc6u, 0x240ca1ccu, 0x2de92c6fu, 0x4a7484aau, 0x5cb0a9dcu, 0x76f988dau,
+      0x983e5152u, 0xa831c66du, 0xb00327c8u, 0xbf597fc7u, 0xc6e00bf3u, 0xd5a79147u, 0x06ca6351u, 0x14292967u,
+      0x27b70a85u, 0x2e1b2138u, 0x4d2c6dfcu, 0x53380d13u, 0x650a7354u, 0x766a0abbu, 0x81c2c92eu, 0x92722c85u,
+      0xa2bfe8a1u, 0xa81a664bu, 0xc24b8b70u, 0xc76c51a3u, 0xd192e819u, 0xd6990624u, 0xf40e3585u, 0x106aa070u,
+      0x19a4c116u, 0x1e376c08u, 0x2748774cu, 0x34b0bcb5u, 0x391c0cb3u, 0x4ed8aa4au, 0x5b9cca4fu, 0x682e6ff3u,
+      0x748f82eeu, 0x78a5636fu, 0x84c87814u, 0x8cc70208u, 0x90befffau, 0xa4506cebu, 0xbef9a3f7u, 0xc67178f2u};
+  return K[i];
+}
+NMSM_HD uint32_t rotr32(uint32_t x, int n) { return (x >> n) | (x << (32 - n)); }
+
+// SHA-256(msg[0..len)) -> out[32], the digest's byte order
+NMSM_HD void sha256(const uint8_t* msg, uint64_t len, uint8_t* out) {
+  uint32_t st[8] = {0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au, 0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u};
+  const uint64_t nblocks = (len + 1 + 8 + 63) / 64;
+  auto byte_at = [&](uint64_t j) -> uint32_t {  // j-th byte of the padded message
+    if (j < len) return msg[j];
+    if (j == len) return 0x80u;
+    const uint64_t end = nblocks * 64;
+    if (j >= end - 8) return (uint32_t)(((len * 8) >> (8 * (end - 1 - j))) & 0xff);  // 64-bit big-endian bit length
+    return 0u;
+  };
+  for (uint64_t b = 0; b < nblocks; b++) {
+    uint32_t w[16];
+    for (int i = 0; i < 16; i++) {
+      uint32_t x = 0;
+      for (int k = 0; k < 4; k++) x = (x << 8) | byte_at(b * 64 + 4 * i + k);
+      w[i] = x;
+    }
+    uint32_t a = st[0], bb = st[1], c = st[2], d = st[3], e = st[4], f = st[5], g = st[6], h = st[7];
+    for (int i = 0; i < 64; i++) {
+      if (i >= 16) {
+        const uint32_t w15 = w[(i - 15) & 15], w2 = w[(i - 2) & 15];
+        const uint32_t s0 = rotr32(w15, 7) ^ rotr32(w15, 18) ^ (w15 >> 3);
+        const uint32_t s1 = rotr32(w2, 17) ^ rotr32(w2, 19) ^ (w2 >> 10);
+        w[i & 15] = w[i & 15] + s0 + w[(i - 7) & 15] + s1;
+      }
+      const uint32_t S1 = rotr32(e, 6) ^ rotr32(e, 11) ^ rotr32(e, 25);
+      const uint32_t ch = (e & f) ^ (~e & g);
+      const uint32_t t1 = h + S1 + ch + sha256_k(i) + w[i & 15];
+      const uint32_t S0 = rotr32(a, 2) ^ rotr32(a, 13) ^ rotr32(a, 22);
+      const uint32_t mj = (a & bb) ^ (a & c) ^ (bb & c);
+      const uint32_t t2 = S0 + mj;
+      h = g; g = f; f = e; e = d + t1; d = c; c = bb; bb = a; a = t1 + t2;
+    }
+    st[0] += a; st[1] += bb; st[2] += c; st[3] += d; st[4] += e; st[5] += f; st[6] += g; st[7] += h;
+  }
+  for (int i = 0; i < 8; i++)
+    for (int k = 0; k < 4; k++) out[4 * i + k] = (uint8_t)(st[i] >> (24 - 8 * k));
+}
+
+// SEC1 uncompressed, 65 B: 04 || x || y, x < p, y < p, on the curve (weierstrass.ts pointFromBytes, `isValidXY`).
+// (0, 0) is rejected although point_on_curve accepts it as the identity encoding: 0 != 0^3 + 7.
+// status as sec1_decode_secp256k1: 0 = invalid, 1 = affine point written (canonical x, y words).
+NMSM_HD int sec1_decode_secp256k1_uncompressed(const uint8_t* enc, uint32_t* out_xy) {
+  if (enc[0] != 0x04) return 0;
+  uint32_t xy[16];
+  words_from_be_bytes<32>(xy, enc + 1);
+  words_from_be_bytes<32>(xy + 8, enc + 33);
+  uint32_t any = 0;
+  for (int k = 0; k < 16; k++) any |= xy[k];
+  if (any == 0 || !point_on_curve<CurveSecp256k1>(xy)) return 0;
+  for (int k = 0; k < 16; k++) out_xy[k] = xy[k];
+  return 1;
+}
+
+NMSM_HD bool words8_nonzero(const uint32_t* a) {
+  uint32_t t = 0;
+  for (int k = 0; k < 8; k++) t |= a[k];
+  return t != 0;
+}
+// a > (n >> 1): the high-S test (Signature.hasHighS)
+NMSM_HD bool ecdsa_high_s(const uint32_t* s) {
+  for (int k = 7; k >= 0; k--) {
+    const uint32_t half = (FnSecp256k1Mod::P(k) >> 1) | (k < 7 ? FnSecp256k1Mod::P(k + 1) << 31 : 0u);
+    if (s[k] != half) return s[k] > half;
+  }
+  return false;
+}
+
+// Signature i: r, s, the public key Q (canonical affine words) and h = bits2int_modN(m).  False = the reference's
+// verify returns false before any scalar multiplication; the outputs are then unspecified.
+NMSM_HD bool ecdsa_prepare_body(uint32_t i, const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off,
+                                const uint8_t* msgs, const uint64_t* msg_off, int flags, uint32_t* q_xy, uint32_t* r,
+                                uint32_t* s, uint32_t* h) {
+  const uint8_t* sig = sigs + (size_t)i * 64;
+  words_from_be_bytes<32>(r, sig);
+  words_from_be_bytes<32>(s, sig + 32);
+  // Signature.fromBytes: 1 <= r < n, 1 <= s < n;  then lowS
+  if (!words8_nonzero(r) || !EcS::canonical_in_range(r) || !words8_nonzero(s) || !EcS::canonical_in_range(s)) return false;
+  if ((flags & ECDSA_LOW_S) && ecdsa_high_s(s)) return false;
+  // Point.fromBytes
+  const uint8_t* pk = pks + pk_off[i];
+  const uint64_t pk_len = pk_off[i + 1] - pk_off[i];
+  if (pk_len == 33) {
+    if (sec1_decode_secp256k1(pk, q_xy) != 1) return false;
+  } else if (pk_len == 65) {
+    if (sec1_decode_secp256k1_uncompressed(pk, q_xy) != 1) return false;
+  } else {
+    return false;
+  }
+  // h = bits2int(m) mod n: the big-endian integer of the first min(len, 32) bytes of m
+  const uint8_t* m = msgs + msg_off[i];
+  uint64_t mlen = msg_off[i + 1] - msg_off[i];
+  uint8_t digest[32];
+  if (flags & ECDSA_PREHASH) {
+    sha256(m, mlen, digest);
+    m = digest;
+    mlen = 32;
+  } else if (mlen > ECDSA_MAX_RAW_MSG) {
+    return false;
+  }
+  const int take = mlen < 32 ? (int)mlen : 32;
+  for (int k = 0; k < 8; k++) h[k] = 0;
+  for (int j = 0; j < take; j++) {
+    const int bit = 8 * (take - 1 - j);
+    h[bit >> 5] |= (uint32_t)m[j] << (bit & 31);
+  }
+  if (!EcS::canonical_in_range(h)) {  // h < 2^256 < 2n: one subtraction reduces it
+    h[0] = sub_cc(h[0], FnSecp256k1Mod::P(0));
+    for (int k = 1; k < 8; k++) h[k] = subc_cc(h[k], FnSecp256k1Mod::P(k));
+  }
+  return true;
+}
+
+// Given w = s^-1 (Montgomery form mod n): u1 = h w, u2 = r w, and the per-signature state k_ecdsa_check reads.
+// ok_out[i] carries the prepare verdict to the check, which overwrites it with the final one.
+NMSM_HD void ecdsa_store(uint32_t i, bool ok, const uint32_t* q_xy, const uint32_t* r, const uint32_t* h, const EcS& w,
+                         uint32_t* qs, uint32_t* u1s, uint32_t* u2s, uint32_t* rs, uint8_t* ok_out) {
+  ok_out[i] = ok ? 1 : 0;
+  if (!ok) return;
+  uint32_t u1[8], u2[8];
+  (EcS::from_canonical(h) * w).to_canonical(u1);
+  (EcS::from_canonical(r) * w).to_canonical(u2);
+  store_words<16>(qs + (size_t)i * 16, q_xy);
+  store_words<8>(u1s + (size_t)i * 8, u1);
+  store_words<8>(u2s + (size_t)i * 8, u2);
+  store_words<8>(rs + (size_t)i * 8, r);
+}
+
+// serial statement of k_ecdsa_prepare (one inversion per signature instead of one per warp)
+NMSM_HD void ecdsa_prepare_serial(uint32_t n, const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off,
+                                  const uint8_t* msgs, const uint64_t* msg_off, int flags, uint32_t* qs, uint32_t* u1s,
+                                  uint32_t* u2s, uint32_t* rs, uint8_t* ok_out) {
+  for (uint32_t i = 0; i < n; i++) {
+    uint32_t q[16], r[8], s[8], h[8];
+    const bool ok = ecdsa_prepare_body(i, sigs, pks, pk_off, msgs, msg_off, flags, q, r, s, h);
+    ecdsa_store(i, ok, q, r, h, ok ? inv(EcS::from_canonical(s)) : EcS::one(), qs, u1s, u2s, rs, ok_out);
+  }
+}
+
+// R.x mod n == r for R = acc (XYZZ, x = X / ZZ), without an inversion: X == r ZZ, or, when r + n < p (R.x >= n is
+// possible because p - n ~ 2^128), X == (r + n) ZZ.  R = O (ZZ = 0) is false.
+NMSM_HD bool ecdsa_x_matches(const typename CurveSecp256k1::G::Acc& acc, const uint32_t* r) {
+  using F = CurveSecp256k1::G::Field;
+  if (CurveSecp256k1::G::is_identity(acc)) return false;
+  if (acc.X == F::from_canonical(r) * acc.ZZ) return true;  // r < n < p
+  uint32_t rn[8];
+  rn[0] = add_cc(r[0], FnSecp256k1Mod::P(0));
+  for (int k = 1; k < 8; k++) rn[k] = addc_cc(r[k], FnSecp256k1Mod::P(k));
+  const uint32_t carry = addc(0, 0);
+  if (carry || !F::canonical_in_range(rn)) return false;
+  return acc.X == F::from_canonical(rn) * acc.ZZ;
+}
+
+// Signature i after ecdsa_store: R = u1 G + u2 Q, out_ok[i] = verdict.  tbl: the fixed-point table of G
+// (table_mul_body layout, BITS-bit digits; BITS is a parameter only so that tests/hostemu can use a small table).
+template <int BITS = PT_BITS>
+NMSM_HD void ecdsa_check_body(uint32_t i, const uint32_t* tbl, const uint32_t* qs, const uint32_t* u1s,
+                              const uint32_t* u2s, const uint32_t* rs, uint8_t* out_ok, unsigned int* err) {
+  using Cv = CurveSecp256k1;
+  using G = Cv::G;
+  if (!out_ok[i]) return;
+  G::Acc acc;
+  table_mul_body<Cv, BITS>(i, tbl, u1s, 1, acc, err);  // u1 < n always; u1 = 0 (h = 0 mod n) gives O
+  uint32_t q[16], u2[8], r[8];
+  load_words<16>(q, qs + (size_t)i * 16);
+  load_words<8>(u2, u2s + (size_t)i * 8);
+  load_words<8>(r, rs + (size_t)i * 8);
+  nl_add<G>(acc, scalar_mul_acc<Cv>(G::prepare(q), u2));  // complete: doubles when u1 G == u2 Q
+  out_ok[i] = ecdsa_x_matches(acc, r) ? 1 : 0;
+}
+
+template <int BITS = PT_BITS>
+NMSM_HD void ecdsa_check_serial(uint32_t n, const uint32_t* tbl, const uint32_t* qs, const uint32_t* u1s,
+                                const uint32_t* u2s, const uint32_t* rs, uint8_t* out_ok, unsigned int* err) {
+  for (uint32_t i = 0; i < n; i++) ecdsa_check_body<BITS>(i, tbl, qs, u1s, u2s, rs, out_ok, err);
+}
+
+}  // namespace nmsm

@@ -873,6 +873,71 @@ def ed25519_verify_batch_packed(sigs: bytes, pks: bytes, msgs: bytes, msg_off: b
     return bool(ok.value), int(bad.value)
 
 
+ECDSA_PREHASH = 1  # include/nmsm.h NMSM_ECDSA_PREHASH
+ECDSA_LOW_S = 2  # include/nmsm.h NMSM_ECDSA_LOW_S
+
+
+def _pack_offsets(items) -> bytes:
+    import struct
+
+    offs = [0]
+    for b in items:
+        offs.append(offs[-1] + len(b))
+    return struct.pack("<%dQ" % len(offs), *offs)
+
+
+def ecdsa_verify_batch(signatures, messages, public_keys, prehash: bool = True, lowS: bool = True) -> List[bool]:
+    """Batch form of secp256k1.verify(sig, msg, publicKey, {prehash, lowS}) with format 'compact' (noble-curves
+    weierstrass.ts ecdsa().verify): one verdict per signature.  Raises where the reference throws before its `try`
+    (non-bytes arguments, a signature that is not 64 bytes) and for lists of different lengths; everything else
+    (r, s out of range, high s, an undecodable key, a raw message over 8192 bytes, R = O) is a False verdict."""
+    n = len(signatures)
+    if len(messages) != n or len(public_keys) != n:
+        raise ValueError("signatures, messages and public keys must have equal length")
+    for what, items in (("signature", signatures), ("message", messages), ("publicKey", public_keys)):
+        for x in items:
+            if not isinstance(x, (bytes, bytearray, memoryview)):
+                raise TypeError('"%s" expected Uint8Array, got type=%s' % (what, type(x).__name__))
+    for s in signatures:
+        if len(s) != 64:
+            raise ValueError('"compact signature" expected Uint8Array of length 64, got length=%d' % len(s))
+    flags = (ECDSA_PREHASH if prehash else 0) | (ECDSA_LOW_S if lowS else 0)
+    out = ecdsa_verify_batch_packed(b"".join(bytes(s) for s in signatures), b"".join(bytes(p) for p in public_keys),
+                                    _pack_offsets(public_keys), b"".join(bytes(m) for m in messages),
+                                    _pack_offsets(messages), n, flags)
+    return [b == 1 for b in out]
+
+
+def ecdsa_verify_batch_packed(sigs: bytes, pks: bytes, pk_off: bytes, msgs: bytes, msg_off: bytes, n: int,
+                              flags: int = ECDSA_PREHASH | ECDSA_LOW_S) -> bytes:
+    """The C-ABI call itself (nmsm_secp256k1_verify_batch) on caller-packed arrays: n*64 signature bytes, the
+    concatenated keys and messages with n+1 little-endian u64 offsets each.  Returns n verdict bytes (1 = valid)."""
+    if len(sigs) != 64 * n or len(pk_off) != 8 * (n + 1) or len(msg_off) != 8 * (n + 1):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    rc = lib.nmsm_secp256k1_verify_batch(cp(sigs or b"\0"), cp(pks or b"\0"), cp(pk_off), cp(msgs or b"\0"),
+                                         cp(msg_off), n, flags, out)
+    try:
+        _lib.check(rc)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return out.raw[:n]
+
+
+def _secp256k1_verify(signature, message, publicKey, prehash: bool = True, lowS: bool = True,
+                      format: str = "compact") -> bool:
+    """secp256k1.verify for one signature (the batch entry point with n = 1)."""
+    if format != "compact":
+        raise NotImplementedError("signature format %r is not part of the accelerated path (compact only)" % (format,))
+    return ecdsa_verify_batch([signature], [message], [publicKey], prehash=prehash, lowS=lowS)[0]
+
+
+secp256k1.verify = _secp256k1_verify
+
+
 DECODE_ZIP215 = 1  # include/nmsm.h NMSM_DECODE_ZIP215
 
 
