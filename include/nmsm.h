@@ -22,6 +22,7 @@
  *                                                                 weierstrass.ts:541-605,971-975, bls12-381.ts:377-468
  *   nmsm_ed25519_verify_batch <- ed25519.verify over a batch      edwards.ts:942-989
  *   nmsm_secp256k1_verify_batch <- secp256k1.verify over a batch, one verdict per signature (weierstrass.ts ecdsa().verify)
+ *   nmsm_secp256k1_schnorr_verify_batch <- schnorr.verify over a batch, one verdict per signature (secp256k1.ts, BIP340)
  *   nmsm_ntt           <- FFT(rootsOfUnity(Fr, G), Fr).direct / .inverse   src/abstract/fft.ts:518-575
  *
  * Data formats (all little-endian, plain bytes, caller-owned):
@@ -217,14 +218,25 @@ int nmsm_ed25519_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const
  * 65-byte uncompressed; message i = msgs[msg_off[i], msg_off[i+1]), any length.  out_ok: n bytes, 1 = valid.
  * Everything about a signature's content (r or s out of [1, n), a high s under NMSM_ECDSA_LOW_S, an undecodable key, a
  * raw message over 8192 bytes, R = O) is a 0 verdict, never an error; NMSM_ERR_ARG is for null pointers, offsets that do
- * not start at 0 or decrease, unknown flag bits and n >= 2^31.  n == 0 writes nothing.  The first call after nmsm_init
- * builds the fixed-point table of G (17 x 2^15 points, 36 MB), kept until nmsm_shutdown.  With profiling on
+ * not start at 0 or decrease, unknown flag bits and n >= 2^31.  n == 0 writes nothing.  The first ECDSA or Schnorr verify
+ * after nmsm_init builds the fixed-point table of G (17 x 2^15 points, 36 MB), kept until nmsm_shutdown.  With profiling on
  * (nmsm_set_profiling), nmsm_last_timing reports k_ecdsa_prepare in slot 0, k_ecdsa_check in slot 1 and both in
  * NMSM_T_TOTAL. */
 #define NMSM_ECDSA_PREHASH 1 /* h = bits2int(sha256(msg_i)) (the reference's default prehash: true) */
 #define NMSM_ECDSA_LOW_S 2   /* s > n/2 verifies false (the reference's default lowS: true for secp256k1) */
 int nmsm_secp256k1_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint64_t* pk_off, const uint8_t* msgs,
                                 const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
+
+/* secp256k1 BIP340 Schnorr batch verification (next-row f6): out_ok[i] = schnorr.verify(sig_i, msg_i, pk_i)
+ * (noble-curves secp256k1.ts), one independent verdict per signature.
+ * sigs: n x 64 B r || s, big-endian; pubkeys: n x 32 B x-only keys; message i = msgs[msg_off[i], msg_off[i+1]), any
+ * length.  out_ok: n bytes, 1 = valid.  Everything about a signature's content (a key x >= p or without a square root,
+ * r >= p, s >= n, r or s zero, R = O, an odd y(R), x(R) != r) is a 0 verdict, never an error; NMSM_ERR_ARG is for null
+ * pointers, offsets that do not start at 0 or decrease, and n >= 2^31.  n == 0 writes nothing.  Shares the fixed-point
+ * table of G with nmsm_secp256k1_verify_batch: whichever verifies first after nmsm_init builds it.  With profiling on,
+ * nmsm_last_timing reports k_schnorr_prepare in slot 0, k_schnorr_check in slot 1 and both in NMSM_T_TOTAL. */
+int nmsm_secp256k1_schnorr_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint8_t* msgs,
+                                        const uint64_t* msg_off, uint64_t n, uint8_t* out_ok);
 
 /* Batched wire-format decoding on the GPU (next-row f2): encodings -> canonical affine points in the packing
  * above, ready for nmsm_msm.  secp256k1: 33-byte SEC1 compressed (weierstrass.ts:565-588); BLS12-381 G1: 48-byte

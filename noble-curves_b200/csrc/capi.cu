@@ -419,8 +419,8 @@ void nmsm_shutdown(void) {
   }
   h2d_release();
   C.ed_scratch.release();
-  cudaFree(C.ecdsa_g_table);
-  C.ecdsa_g_table = nullptr;
+  cudaFree(C.secp256k1_g_table);
+  C.secp256k1_g_table = nullptr;
   for (Buf* b : {&C.ntt_data, &C.ntt_work, &C.ntt_tmp, &C.ntt_roots, &C.ntt_aux}) b->release();
   C.ntt_key_field = -1;
   C.ntt_key_bits = -1;
@@ -771,6 +771,18 @@ int nmsm_secp256k1_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, con
   if (!sigs || !pk_off || !msg_off || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
   if ((pk_off[n] && !pubkeys) || (msg_off[n] && !msgs)) return fail(NMSM_ERR_ARG, "null pointer");
   return secp256k1_verify_batch_impl(sigs, pubkeys, pk_off, msgs, msg_off, n, flags, out_ok);
+}
+
+int nmsm_secp256k1_schnorr_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint8_t* msgs,
+                                        const uint64_t* msg_off, uint64_t n, uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (n == 0) return NMSM_OK;
+  if (!sigs || !pubkeys || !msg_off || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
+  if (msg_off[n] && !msgs) return fail(NMSM_ERR_ARG, "null pointer");
+  return secp256k1_schnorr_verify_batch_impl(sigs, pubkeys, msgs, msg_off, n, out_ok);
 }
 
 int nmsm_points_decode_ex(int curve, const uint8_t* enc, uint64_t n, int flags, uint8_t* out_xy, uint8_t* out_status) {

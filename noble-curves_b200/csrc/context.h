@@ -99,7 +99,7 @@ struct Context {
   Slot slot[NUM_SLOTS];
   int cur = 0;  // slot used by the call in progress (set by the C-ABI wrapper under the mutex)
   Buf ed_scratch;              // signature-verification scratch (ed25519 and secp256k1 batches)
-  uint32_t* ecdsa_g_table = nullptr;  // fixed-point table of the secp256k1 generator, built by the first ECDSA verify
+  uint32_t* secp256k1_g_table = nullptr;  // fixed-point table of the secp256k1 generator, built by the first verify
   Buf ntt_data, ntt_work, ntt_tmp, ntt_roots, ntt_aux;  // NTT staging / work / output / root table (ntt.cu)
   int ntt_key_field = -1, ntt_key_bits = -1;            // which root table ntt_roots holds
   uint64_t ntt_key_gen = 0;
@@ -206,6 +206,8 @@ int ed25519_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uin
                               uint64_t n, const uint8_t* z16, int* out_ok, long long* out_bad_index);
 int secp256k1_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off, const uint8_t* msgs,
                                 const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
+int secp256k1_schnorr_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs,
+                                        const uint64_t* msg_off, uint64_t n, uint8_t* out_ok);
 int decode_points_impl(int curve, const uint8_t* enc, uint64_t n, int flags, uint8_t* out_xy, uint8_t* out_status);
 int ntt_impl(int curve, void* values, int on_device, int log_n, uint64_t generator, int inverse, int brp_input,
              int brp_output);

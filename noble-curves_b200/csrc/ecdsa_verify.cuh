@@ -40,44 +40,56 @@ NMSM_HD uint32_t sha256_k(int i) {
 }
 NMSM_HD uint32_t rotr32(uint32_t x, int n) { return (x >> n) | (x << (32 - n)); }
 
-// SHA-256(msg[0..len)) -> out[32], the digest's byte order
-NMSM_HD void sha256(const uint8_t* msg, uint64_t len, uint8_t* out) {
-  uint32_t st[8] = {0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au, 0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u};
+// One SHA-256 compression: st <- st + the 64 rounds over the block w[16] (big-endian words; w is overwritten).
+NMSM_HD void sha256_compress(uint32_t* st, uint32_t* w) {
+  uint32_t a = st[0], bb = st[1], c = st[2], d = st[3], e = st[4], f = st[5], g = st[6], h = st[7];
+  for (int i = 0; i < 64; i++) {
+    if (i >= 16) {
+      const uint32_t w15 = w[(i - 15) & 15], w2 = w[(i - 2) & 15];
+      const uint32_t s0 = rotr32(w15, 7) ^ rotr32(w15, 18) ^ (w15 >> 3);
+      const uint32_t s1 = rotr32(w2, 17) ^ rotr32(w2, 19) ^ (w2 >> 10);
+      w[i & 15] = w[i & 15] + s0 + w[(i - 7) & 15] + s1;
+    }
+    const uint32_t S1 = rotr32(e, 6) ^ rotr32(e, 11) ^ rotr32(e, 25);
+    const uint32_t ch = (e & f) ^ (~e & g);
+    const uint32_t t1 = h + S1 + ch + sha256_k(i) + w[i & 15];
+    const uint32_t S0 = rotr32(a, 2) ^ rotr32(a, 13) ^ rotr32(a, 22);
+    const uint32_t mj = (a & bb) ^ (a & c) ^ (bb & c);
+    const uint32_t t2 = S0 + mj;
+    h = g; g = f; f = e; e = d + t1; d = c; c = bb; bb = a; a = t1 + t2;
+  }
+  st[0] += a; st[1] += bb; st[2] += c; st[3] += d; st[4] += e; st[5] += f; st[6] += g; st[7] += h;
+}
+
+// Finish a SHA-256 whose first `done` bytes (a multiple of 64) are already compressed into st: absorb the `len` bytes
+// byte_at(0 .. len), pad for a total of done + len bytes, and write the digest (its byte order) to out[32].
+template <class ByteAt>
+NMSM_HD void sha256_finish(uint32_t* st, uint64_t done, uint64_t len, const ByteAt& byte_at, uint8_t* out) {
   const uint64_t nblocks = (len + 1 + 8 + 63) / 64;
-  auto byte_at = [&](uint64_t j) -> uint32_t {  // j-th byte of the padded message
-    if (j < len) return msg[j];
+  const uint64_t end = nblocks * 64, bits = (done + len) * 8;
+  auto padded = [&](uint64_t j) -> uint32_t {  // j-th byte of the padded tail
+    if (j < len) return byte_at(j);
     if (j == len) return 0x80u;
-    const uint64_t end = nblocks * 64;
-    if (j >= end - 8) return (uint32_t)(((len * 8) >> (8 * (end - 1 - j))) & 0xff);  // 64-bit big-endian bit length
+    if (j >= end - 8) return (uint32_t)((bits >> (8 * (end - 1 - j))) & 0xff);  // 64-bit big-endian bit length
     return 0u;
   };
   for (uint64_t b = 0; b < nblocks; b++) {
     uint32_t w[16];
     for (int i = 0; i < 16; i++) {
       uint32_t x = 0;
-      for (int k = 0; k < 4; k++) x = (x << 8) | byte_at(b * 64 + 4 * i + k);
+      for (int k = 0; k < 4; k++) x = (x << 8) | padded(b * 64 + 4 * i + k);
       w[i] = x;
     }
-    uint32_t a = st[0], bb = st[1], c = st[2], d = st[3], e = st[4], f = st[5], g = st[6], h = st[7];
-    for (int i = 0; i < 64; i++) {
-      if (i >= 16) {
-        const uint32_t w15 = w[(i - 15) & 15], w2 = w[(i - 2) & 15];
-        const uint32_t s0 = rotr32(w15, 7) ^ rotr32(w15, 18) ^ (w15 >> 3);
-        const uint32_t s1 = rotr32(w2, 17) ^ rotr32(w2, 19) ^ (w2 >> 10);
-        w[i & 15] = w[i & 15] + s0 + w[(i - 7) & 15] + s1;
-      }
-      const uint32_t S1 = rotr32(e, 6) ^ rotr32(e, 11) ^ rotr32(e, 25);
-      const uint32_t ch = (e & f) ^ (~e & g);
-      const uint32_t t1 = h + S1 + ch + sha256_k(i) + w[i & 15];
-      const uint32_t S0 = rotr32(a, 2) ^ rotr32(a, 13) ^ rotr32(a, 22);
-      const uint32_t mj = (a & bb) ^ (a & c) ^ (bb & c);
-      const uint32_t t2 = S0 + mj;
-      h = g; g = f; f = e; e = d + t1; d = c; c = bb; bb = a; a = t1 + t2;
-    }
-    st[0] += a; st[1] += bb; st[2] += c; st[3] += d; st[4] += e; st[5] += f; st[6] += g; st[7] += h;
+    sha256_compress(st, w);
   }
   for (int i = 0; i < 8; i++)
     for (int k = 0; k < 4; k++) out[4 * i + k] = (uint8_t)(st[i] >> (24 - 8 * k));
+}
+
+// SHA-256(msg[0..len)) -> out[32], the digest's byte order
+NMSM_HD void sha256(const uint8_t* msg, uint64_t len, uint8_t* out) {
+  uint32_t st[8] = {0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au, 0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u};
+  sha256_finish(st, 0, len, [&](uint64_t j) -> uint32_t { return msg[j]; }, out);
 }
 
 // SEC1 uncompressed, 65 B: 04 || x || y, x < p, y < p, on the curve (weierstrass.ts pointFromBytes, `isValidXY`).

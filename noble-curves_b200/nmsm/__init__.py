@@ -938,6 +938,53 @@ def _secp256k1_verify(signature, message, publicKey, prehash: bool = True, lowS:
 secp256k1.verify = _secp256k1_verify
 
 
+def schnorr_verify_batch(signatures, messages, public_keys) -> List[bool]:
+    """Batch form of schnorr.verify(signature, message, publicKey) (noble-curves secp256k1.ts, BIP340): one verdict
+    per signature.  Raises where the reference throws before its `try` (non-bytes arguments, a signature that is not 64
+    bytes, a key that is not 32 bytes) and for lists of different lengths; everything else (a key that is not an x
+    coordinate on the curve, r >= p, s >= n, R = O, an odd y(R), x(R) != r) is a False verdict."""
+    n = len(signatures)
+    if len(messages) != n or len(public_keys) != n:
+        raise ValueError("signatures, messages and public keys must have equal length")
+    for what, items in (("signature", signatures), ("message", messages), ("publicKey", public_keys)):
+        for x in items:
+            if not isinstance(x, (bytes, bytearray, memoryview)):
+                raise TypeError('"%s" expected Uint8Array, got type=%s' % (what, type(x).__name__))
+    for what, items, size in (("signature", signatures, 64), ("publicKey", public_keys, 32)):
+        for x in items:
+            if len(x) != size:
+                raise ValueError('"%s" expected Uint8Array of length %d, got length=%d' % (what, size, len(x)))
+    out = schnorr_verify_batch_packed(b"".join(bytes(s) for s in signatures), b"".join(bytes(p) for p in public_keys),
+                                      b"".join(bytes(m) for m in messages), _pack_offsets(messages), n)
+    return [b == 1 for b in out]
+
+
+def schnorr_verify_batch_packed(sigs: bytes, pks: bytes, msgs: bytes, msg_off: bytes, n: int) -> bytes:
+    """The C-ABI call itself (nmsm_secp256k1_schnorr_verify_batch) on caller-packed arrays: n*64 signature bytes, n*32
+    x-only key bytes, the concatenated messages with n+1 little-endian u64 offsets.  Returns n verdict bytes (1 = valid)."""
+    if len(sigs) != 64 * n or len(pks) != 32 * n or len(msg_off) != 8 * (n + 1):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    rc = lib.nmsm_secp256k1_schnorr_verify_batch(cp(sigs or b"\0"), cp(pks or b"\0"), cp(msgs or b"\0"), cp(msg_off), n,
+                                                 out)
+    try:
+        _lib.check(rc)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return out.raw[:n]
+
+
+def _schnorr_verify(signature, message, publicKey) -> bool:
+    """schnorr.verify for one signature (the batch entry point with n = 1)."""
+    return schnorr_verify_batch([signature], [message], [publicKey])[0]
+
+
+schnorr = _NS(verify=_schnorr_verify)  # the reference's `schnorr` export (secp256k1.ts)
+
+
 DECODE_ZIP215 = 1  # include/nmsm.h NMSM_DECODE_ZIP215
 
 
