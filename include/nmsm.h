@@ -238,6 +238,34 @@ int nmsm_secp256k1_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, con
 int nmsm_secp256k1_schnorr_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint8_t* msgs,
                                         const uint64_t* msg_off, uint64_t n, uint8_t* out_ok);
 
+/* BLS12-381 batch pairing checks (next-row f7): out_ok[j] = 1 iff prod_{i in [pair_off[j], pair_off[j+1])} e(P_i, Q_i)
+ * == 1 in GT, the optimal-ate pairing of the reference (src/abstract/bls.ts, bls12-381.ts), one verdict per check.
+ * g1_xy: P_i in the affine packing above (96 B: x, y); g2_xy: Q_i (192 B: x.c0, x.c1, y.c0, y.c1), each coordinate 48 B
+ * little-endian; pair_off: n_checks + 1 offsets, the pair count is pair_off[n_checks].  An empty check is 1.  A pair
+ * with an identity point ((0, 0)) contributes 1, its mathematical value; the reference's pairing throws on the zero
+ * point instead.  Points are NOT subgroup-checked (as for the MSM ids 4 and 5; nmsm_points_torsion_free does that):
+ * outside the subgroups the verdict is whatever the same formulas give.  NMSM_ERR_POINT, with nmsm_last_error_index =
+ * the pair index, for a coordinate >= p or a point off its curve (every G1 point is checked before any G2 point);
+ * NMSM_ERR_ARG for null pointers, offsets that do not start at 0 or decrease, and 2^31 or more pairs.  n_checks == 0
+ * writes nothing.  Miller loops run in chunks of 2^16 pairs (a 38 MB workspace).  With profiling on,
+ * nmsm_last_timing reports k_bls_miller in slot 0, k_bls_final in slot 1 (each summed over the chunks) and their sum
+ * in NMSM_T_TOTAL. */
+int nmsm_bls12_381_pairing_check_batch(const uint8_t* g1_xy, const uint8_t* g2_xy, const uint64_t* pair_off,
+                                       uint64_t n_checks, uint8_t* out_ok);
+
+/* BLS12-381 batch signature verification (next-row f7): out_ok[i] = bls12_381.verify(sig_i, H_i, pk_i) for long
+ * signatures (public key in G1, signature in G2), one independent verdict per signature.
+ * sigs96: n x 96 B Zcash-flag compressed G2 signatures; pks48: n x 48 B Zcash-flag compressed G1 keys; msg_pts: n x
+ * 192 B messages ALREADY HASHED to G2, in the affine G2 packing (hash-to-curve is not part of the library).
+ * out_ok[i] = 1 iff pk decodes, is not the identity and is in G1, sig decodes, is not the identity and is in G2, H is
+ * not the identity, and e(pk, H) e(-G1, sig) == 1.  Everything about a signature's or key's content is a 0 verdict,
+ * never an error.  H comes from the caller's hash-to-curve and is in G2 by construction, so it is only checked for
+ * range and curve: NMSM_ERR_POINT with nmsm_last_error_index = i for an H with a coordinate >= p or off the twist.
+ * NMSM_ERR_ARG for null pointers and n >= 2^30.  n == 0 writes nothing.  With profiling on, nmsm_last_timing reports
+ * k_bls_verify_prepare in slot 0, k_bls_miller in slot 1, k_bls_final in slot 2 and their sum in NMSM_T_TOTAL. */
+int nmsm_bls12_381_verify_batch(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msg_pts, uint64_t n,
+                                uint8_t* out_ok);
+
 /* Batched wire-format decoding on the GPU (next-row f2): encodings -> canonical affine points in the packing
  * above, ready for nmsm_msm.  secp256k1: 33-byte SEC1 compressed (weierstrass.ts:565-588); BLS12-381 G1: 48-byte
  * Zcash-flag compressed (bls12-381.ts:377-468); BLS12-381 G2: 96-byte Zcash-flag compressed, x = c1 || c0

@@ -985,6 +985,122 @@ def _schnorr_verify(signature, message, publicKey) -> bool:
 schnorr = _NS(verify=_schnorr_verify)  # the reference's `schnorr` export (secp256k1.ts)
 
 
+# ---- BLS12-381 pairing checks and BLS signatures (include/nmsm.h nmsm_bls12_381_*) -----------------------------------
+def _bls_g2_compress(pt) -> bytes:
+    """Zcash-flag compressed G2 encoding (bls12-381.ts:377-402,488-491): x.c1 || x.c0 big-endian, sort bit over
+    [y.c1, y.c0]."""
+    if pt.is0():
+        return bytes([0xC0]) + bytes(95)
+    (x0, x1), (y0, y1) = pt.x, pt.y
+    b = bytearray(x1.to_bytes(48, "big") + x0.to_bytes(48, "big"))
+    part = y1 if y1 else y0
+    b[0] |= 0x80 | (0x20 if (part * 2) // _BLS_P else 0)
+    return bytes(b)
+
+
+def pairing_check_batch(checks) -> List[bool]:
+    """One verdict per check: checks[j] is a list of (G1 Point, G2 Point) pairs, True iff the product of their pairings
+    is 1 (noble's pairingBatch compared with Fp12.ONE).  A pair with an identity point contributes 1 (the reference
+    throws on the zero point); points are not subgroup-checked (assertValidity / isTorsionFree does that).  Raises
+    ValueError for a point off its curve."""
+    G1, G2 = bls12_381.G1.Point, bls12_381.G2.Point
+    g1, g2, offs = [], [], [0]
+    for j, check in enumerate(checks):
+        for pair in check:
+            if len(pair) != 2 or not isinstance(pair[0], G1) or not isinstance(pair[1], G2):
+                raise TypeError("check %d: (bls12_381.G1.Point, bls12_381.G2.Point) pairs expected" % j)
+            g1.append(pair[0])
+            g2.append(pair[1])
+        offs.append(len(g1))
+    import struct
+
+    try:
+        out = pairing_check_batch_packed(_pack_points(g1), _pack_points(g2), struct.pack("<%dQ" % len(offs), *offs),
+                                         len(checks))
+    except NmsmError as e:
+        _raise_mapped(e)
+    return [b == 1 for b in out]
+
+
+def pairing_check_batch_packed(g1_xy: bytes, g2_xy: bytes, pair_off: bytes, n_checks: int) -> bytes:
+    """The C-ABI call itself (nmsm_bls12_381_pairing_check_batch): packed affine G1 (96 B) and G2 (192 B) points and
+    n_checks + 1 little-endian u64 pair offsets.  Returns n_checks verdict bytes; raises NmsmError (with .code and
+    .index) on an error."""
+    if len(pair_off) != 8 * (n_checks + 1):
+        raise ValueError("packed arrays do not match n_checks")
+    total = int.from_bytes(pair_off[-8:], "little") if n_checks else 0
+    if len(g1_xy) != 96 * total or len(g2_xy) != 192 * total:
+        raise ValueError("packed arrays do not match the pair count")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n_checks, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    _lib.check(lib.nmsm_bls12_381_pairing_check_batch(cp(g1_xy or b"\0"), cp(g2_xy or b"\0"), cp(pair_off), n_checks,
+                                                      out))
+    return out.raw[:n_checks]
+
+
+def bls_verify_batch(signatures, message_points, public_keys) -> List[bool]:
+    """Batch form of bls12_381.verify(signature, message, publicKey) for long signatures (public key in G1, signature in
+    G2): one verdict per signature.  Signatures are 96-byte and keys 48-byte Zcash-flag compressed encodings, or Points
+    (encoded first).  Messages must already be hashed to G2 (bls12_381.G2.Point): hash-to-curve is not implemented, so
+    bytes messages raise.  A signature or key that does not decode, is the identity or lies outside its subgroup is a
+    False verdict; a message point off the curve raises ValueError."""
+    n = len(signatures)
+    if len(message_points) != n or len(public_keys) != n:
+        raise ValueError("signatures, messages and public keys must have equal length")
+    G1, G2 = bls12_381.G1.Point, bls12_381.G2.Point
+    sigs, pks = [], []
+    for s in signatures:
+        if isinstance(s, G2):
+            s = _bls_g2_compress(s)
+        if not isinstance(s, (bytes, bytearray, memoryview)):
+            raise TypeError('"signature" expected Uint8Array or G2 Point, got type=%s' % type(s).__name__)
+        if len(s) != 96:
+            raise ValueError('"signature" expected Uint8Array of length 96, got length=%d' % len(s))
+        sigs.append(bytes(s))
+    for k in public_keys:
+        if isinstance(k, G1):
+            k = k.toBytes(True)
+        if not isinstance(k, (bytes, bytearray, memoryview)):
+            raise TypeError('"publicKey" expected Uint8Array or G1 Point, got type=%s' % type(k).__name__)
+        if len(k) != 48:
+            raise ValueError('"publicKey" expected Uint8Array of length 48, got length=%d' % len(k))
+        pks.append(bytes(k))
+    for m in message_points:
+        if isinstance(m, (bytes, bytearray, memoryview, str)):
+            raise NotImplementedError("hash-to-curve is not implemented: pass the message hashed to G2 as a "
+                                      "bls12_381.G2.Point")
+        if not isinstance(m, G2):
+            raise TypeError('"message" expected bls12_381.G2.Point, got type=%s' % type(m).__name__)
+    try:
+        out = bls_verify_batch_packed(b"".join(sigs), b"".join(pks), _pack_points(message_points), n)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return [b == 1 for b in out]
+
+
+def bls_verify_batch_packed(sigs96: bytes, pks48: bytes, msg_pts: bytes, n: int) -> bytes:
+    """The C-ABI call itself (nmsm_bls12_381_verify_batch): n*96 signature bytes, n*48 key bytes and n*192 bytes of
+    affine G2 message points.  Returns n verdict bytes; raises NmsmError (with .code and .index) on an error."""
+    if len(sigs96) != 96 * n or len(pks48) != 48 * n or len(msg_pts) != 192 * n:
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    _lib.check(lib.nmsm_bls12_381_verify_batch(cp(sigs96 or b"\0"), cp(pks48 or b"\0"), cp(msg_pts or b"\0"), n, out))
+    return out.raw[:n]
+
+
+def _bls_verify(signature, message, publicKey) -> bool:
+    """bls12_381.verify for one signature (the batch entry point with n = 1)."""
+    return bls_verify_batch([signature], [message], [publicKey])[0]
+
+
+bls12_381.verify = _bls_verify
+
+
 DECODE_ZIP215 = 1  # include/nmsm.h NMSM_DECODE_ZIP215
 
 
