@@ -23,6 +23,7 @@
  *   nmsm_ed25519_verify_batch <- ed25519.verify over a batch      edwards.ts:942-989
  *   nmsm_secp256k1_verify_batch <- secp256k1.verify over a batch, one verdict per signature (weierstrass.ts ecdsa().verify)
  *   nmsm_secp256k1_schnorr_verify_batch <- schnorr.verify over a batch, one verdict per signature (secp256k1.ts, BIP340)
+ *   nmsm_bls12_381_pairing_check_batch / nmsm_bn254_pairing_check_batch <- pairingBatch(...) == 1, one verdict per check
  *   nmsm_ntt           <- FFT(rootsOfUnity(Fr, G), Fr).direct / .inverse   src/abstract/fft.ts:518-575
  *
  * Data formats (all little-endian, plain bytes, caller-owned):
@@ -252,6 +253,20 @@ int nmsm_secp256k1_schnorr_verify_batch(const uint8_t* sigs, const uint8_t* pubk
  * in NMSM_T_TOTAL. */
 int nmsm_bls12_381_pairing_check_batch(const uint8_t* g1_xy, const uint8_t* g2_xy, const uint64_t* pair_off,
                                        uint64_t n_checks, uint8_t* out_ok);
+
+/* bn254 batch pairing checks (next-row f8): the contract of nmsm_bls12_381_pairing_check_batch on bn254 (the
+ * reference's bn254.pairing / pairingBatch; Ethereum's ecPairing precompile, EIP-197; Groth16 and KZG verification).
+ * out_ok[j] = 1 iff prod_{i in [pair_off[j], pair_off[j+1])} e(P_i, Q_i) == 1 in GT, the optimal-ate pairing.
+ * g1_xy: P_i in the affine packing above (64 B: x, y); g2_xy: Q_i (128 B: x.c0, x.c1, y.c0, y.c1), each coordinate 32 B
+ * little-endian (the NMSM_BN254_G1 / G2 packing).  An empty check is 1; a pair with an identity point ((0, 0))
+ * contributes 1.  Points are NOT subgroup-checked (nmsm_points_torsion_free(NMSM_BN254_G2, ...) does that; EIP-197
+ * requires it for G2).  NMSM_ERR_POINT, with nmsm_last_error_index = the pair index, for a coordinate >= p or a point
+ * off its curve (every G1 point is checked before any G2 point); NMSM_ERR_ARG for null pointers, offsets that do not
+ * start at 0 or decrease, and 2^31 or more checks or pairs.  n_checks == 0 writes nothing.  Miller loops run in chunks
+ * of 2^16 pairs (a 25 MB workspace).  With profiling on, nmsm_last_timing reports k_bn254_miller in slot 0,
+ * k_bn254_final in slot 1 (each summed over the chunks) and their sum in NMSM_T_TOTAL. */
+int nmsm_bn254_pairing_check_batch(const uint8_t* g1_xy, const uint8_t* g2_xy, const uint64_t* pair_off,
+                                   uint64_t n_checks, uint8_t* out_ok);
 
 /* BLS12-381 batch signature verification (next-row f7): out_ok[i] = bls12_381.verify(sig_i, H_i, pk_i) for long
  * signatures (public key in G1, signature in G2), one independent verdict per signature.

@@ -796,6 +796,17 @@ int nmsm_bls12_381_pairing_check_batch(const uint8_t* g1_xy, const uint8_t* g2_x
   return bls12_381_pairing_check_batch_impl(g1_xy, g2_xy, pair_off, n_checks, out_ok);
 }
 
+int nmsm_bn254_pairing_check_batch(const uint8_t* g1_xy, const uint8_t* g2_xy, const uint64_t* pair_off,
+                                   uint64_t n_checks, uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (n_checks == 0) return NMSM_OK;
+  if (!pair_off || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
+  return bn254_pairing_check_batch_impl(g1_xy, g2_xy, pair_off, n_checks, out_ok);
+}
+
 int nmsm_bls12_381_verify_batch(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msg_pts, uint64_t n,
                                 uint8_t* out_ok) {
   std::lock_guard<std::mutex> lk(g_mu);

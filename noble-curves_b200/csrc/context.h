@@ -210,6 +210,8 @@ int secp256k1_schnorr_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks,
                                         const uint64_t* msg_off, uint64_t n, uint8_t* out_ok);
 int bls12_381_pairing_check_batch_impl(const uint8_t* g1_xy, const uint8_t* g2_xy, const uint64_t* pair_off,
                                        uint64_t n_checks, uint8_t* out_ok);
+int bn254_pairing_check_batch_impl(const uint8_t* g1_xy, const uint8_t* g2_xy, const uint64_t* pair_off,
+                                   uint64_t n_checks, uint8_t* out_ok);
 int bls12_381_verify_batch_impl(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msg_pts, uint64_t n,
                                 uint8_t* out_ok);
 int decode_points_impl(int curve, const uint8_t* enc, uint64_t n, int flags, uint8_t* out_xy, uint8_t* out_status);

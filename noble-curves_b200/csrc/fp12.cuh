@@ -1,13 +1,14 @@
-// The pairing tower over the BLS12-381 base field (SURVEY §8 row f7), the reference's src/abstract/tower.ts:
-//   Fp6  = Fp2[v]/(v^3 - xi),  xi = 1 + u
+// The pairing towers over the BLS12-381 and bn254 base fields (SURVEY §8 rows f7, f8), the reference's
+// src/abstract/tower.ts:
+//   Fp6  = Fp2[v]/(v^3 - xi),  xi = 1 + u (BLS12-381), 9 + u (bn254)
 //   Fp12 = Fp6[w]/(w^2 - v)
 // An Fp12 element is c0 + c1 w with c0, c1 in Fp6; an Fp6 element is c0 + c1 v + c2 v^2 with coefficients in Fp2.  The
-// memory order (c0.c0.c0, c0.c0.c1, c0.c1.c0, ..., c1.c2.c1; 12 Fp values of 12 words, Montgomery form) is the order
+// memory order (c0.c0.c0, c0.c0.c1, c0.c1.c0, ..., c1.c2.c1; 12 Fp values of N words, Montgomery form) is the order
 // the pairing workspace and tests/hostemu use.
 //
-// The tower is a template over a policy T (field parameters, multiplication by xi, Frobenius coefficients) so that a
-// second curve's tower is a new policy; only Bls381Tower exists.  The heavy operations are out of line on the device
-// (NMSM_HD_NOINLINE): one copy of each body keeps the pairing kernels' code size and ptxas time reasonable.
+// The tower is a template over a policy T (field parameters, multiplication by xi, Frobenius coefficients, the curve
+// parameter x of the cyclotomic exponentiation): Bls381Tower and Bn254Tower.  The heavy operations are out of line on
+// the device (NMSM_HD_NOINLINE): one copy of each body keeps the pairing kernels' code size and ptxas time reasonable.
 #pragma once
 #include "curve_consts.cuh"
 #include "fp2.cuh"
@@ -20,35 +21,61 @@ namespace nmsm {
 #define NMSM_HD_NOINLINE inline
 #endif
 
+// Frobenius^K coefficients of a generated block Fr (tools/gen_consts.py Bls381Frob, Bn254Frob):
+// v -> c1 v, v^2 -> c2 v^2, w -> cw w
+template <class Fr, int K, class F2>
+NMSM_HD void frob_coeffs_from(F2& c1, F2& c2, F2& cw) {
+#define NMSM_FROB_LD(dst, NAME)          \
+  dst.c0.v[i] = Fr::NAME##_C0_MONT(i); \
+  dst.c1.v[i] = Fr::NAME##_C1_MONT(i)
+  for (int i = 0; i < F2::Params::N; i++) {
+    if constexpr (K == 1) {
+      NMSM_FROB_LD(c1, FROB6_C1_1);
+      NMSM_FROB_LD(c2, FROB6_C2_1);
+      NMSM_FROB_LD(cw, FROB12_C1_1);
+    } else if constexpr (K == 2) {
+      NMSM_FROB_LD(c1, FROB6_C1_2);
+      NMSM_FROB_LD(c2, FROB6_C2_2);
+      NMSM_FROB_LD(cw, FROB12_C1_2);
+    } else {
+      static_assert(K == 3, "Frobenius powers 1..3");
+      NMSM_FROB_LD(c1, FROB6_C1_3);
+      NMSM_FROB_LD(c2, FROB6_C2_3);
+      NMSM_FROB_LD(cw, FROB12_C1_3);
+    }
+  }
+#undef NMSM_FROB_LD
+}
+
 struct Bls381Tower {
   using C = FpBls381;
   using F = Fp<FpBls381>;
   using F2 = Fp2<FpBls381>;
   NMSM_HD static F2 mul_by_xi(const F2& a) { return F2{a.c0 - a.c1, a.c0 + a.c1}; }  // (a0 + a1 u)(1 + u)
-  // Frobenius^K coefficients (tools/gen_consts.py Bls381Frob): v -> c1 v, v^2 -> c2 v^2, w -> cw w
   template <int K>
   NMSM_HD static void frob_coeffs(F2& c1, F2& c2, F2& cw) {
-#define NMSM_FROB_LD(dst, NAME)                  \
-  dst.c0.v[i] = Bls381Frob::NAME##_C0_MONT(i); \
-  dst.c1.v[i] = Bls381Frob::NAME##_C1_MONT(i)
-    for (int i = 0; i < 12; i++) {
-      if constexpr (K == 1) {
-        NMSM_FROB_LD(c1, FROB6_C1_1);
-        NMSM_FROB_LD(c2, FROB6_C2_1);
-        NMSM_FROB_LD(cw, FROB12_C1_1);
-      } else if constexpr (K == 2) {
-        NMSM_FROB_LD(c1, FROB6_C1_2);
-        NMSM_FROB_LD(c2, FROB6_C2_2);
-        NMSM_FROB_LD(cw, FROB12_C1_2);
-      } else {
-        static_assert(K == 3, "Frobenius powers 1..3");
-        NMSM_FROB_LD(c1, FROB6_C1_3);
-        NMSM_FROB_LD(c2, FROB6_C2_3);
-        NMSM_FROB_LD(cw, FROB12_C1_3);
-      }
-    }
-#undef NMSM_FROB_LD
+    frob_coeffs_from<Bls381Frob, K>(c1, c2, cw);
   }
+  // |x| = Bls381G2Gls::Z = 0xd201000000010000, the exponent of fp12_cyclotomic_exp_x
+  static constexpr int X_BITS = 64;
+  NMSM_HD static constexpr uint32_t X(int i) { return Bls381G2Gls::Z(i); }
+};
+
+struct Bn254Tower {
+  using C = FpBn254;
+  using F = Fp<FpBn254>;
+  using F2 = Fp2<FpBn254>;
+  NMSM_HD static F2 mul_by_xi(const F2& a) {  // (a0 + a1 u)(9 + u) = (9 a0 - a1) + (a0 + 9 a1) u
+    const F2 a2 = a + a, a4 = a2 + a2, a9 = a4 + a4 + a;
+    return F2{a9.c0 - a.c1, a.c0 + a9.c1};
+  }
+  template <int K>
+  NMSM_HD static void frob_coeffs(F2& c1, F2& c2, F2& cw) {
+    frob_coeffs_from<Bn254Frob, K>(c1, c2, cw);
+  }
+  // u = Bn254Ate::U = 0x44e992b44a6909f1, the exponent of fp12_cyclotomic_exp_x
+  static constexpr int X_BITS = Bn254Ate::U_BITS;
+  NMSM_HD static constexpr uint32_t X(int i) { return Bn254Ate::U(i); }
 };
 
 template <class T>
@@ -160,6 +187,16 @@ NMSM_HD_NOINLINE Fp12<T> fp12_mul_by_014(const Fp12<T>& f, const typename T::F2&
   return Fp12<T>{t0 + fp6_mul_by_v(t1), s - t0 - t1};
 }
 
+// f * (l0 + l3 w + l4 v w): the sparse shape of a Miller-loop line on the D-type twist (pairing_bn254.cuh)
+template <class T>
+NMSM_HD_NOINLINE Fp12<T> fp12_mul_by_034(const Fp12<T>& f, const typename T::F2& l0, const typename T::F2& l3,
+                                         const typename T::F2& l4) {
+  using F6 = Fp6<T>;
+  const F6 t0{f.c0.c0 * l0, f.c0.c1 * l0, f.c0.c2 * l0}, t1 = fp6_mul_by_01(f.c1, l3, l4);
+  const F6 s = fp6_mul_by_01(f.c0 + f.c1, l0 + l3, l4);
+  return Fp12<T>{t0 + fp6_mul_by_v(t1), s - t0 - t1};
+}
+
 template <class T>
 NMSM_HD Fp12<T> fp12_conj(const Fp12<T>& a) {  // a^(p^6): w -> -w
   return Fp12<T>{a.c0, -a.c1};
@@ -219,13 +256,14 @@ NMSM_HD_NOINLINE Fp12<T> fp12_cyclotomic_sqr(const Fp12<T>& f) {
   return Fp12<T>{Fp6<T>{z0, z4, z3}, Fp6<T>{z2, z1, z5}};
 }
 
-// a^|x| in the cyclotomic subgroup, |x| = Bls381G2Gls::Z = 0xd201000000010000: 63 squarings, 5 multiplications
+// a^x in the cyclotomic subgroup for the policy's exponent x = T::X (a top bit and X_BITS - 1 more): X_BITS - 1
+// squarings and one multiplication per further set bit (BLS12-381 |x|: 63 and 5; bn254 u: 62 and 27)
 template <class T>
 NMSM_HD_NOINLINE Fp12<T> fp12_cyclotomic_exp_x(const Fp12<T>& a) {
   Fp12<T> r = a;
-  for (int i = 62; i >= 0; i--) {
+  for (int i = T::X_BITS - 2; i >= 0; i--) {
     r = fp12_cyclotomic_sqr(r);
-    const uint32_t bit = i >= 32 ? (Bls381G2Gls::Z(1) >> (i - 32)) & 1u : (Bls381G2Gls::Z(0) >> i) & 1u;
+    const uint32_t bit = i >= 32 ? (T::X(1) >> (i - 32)) & 1u : (T::X(0) >> i) & 1u;
     if (bit) r = fp12_mul(r, a);
   }
   return r;

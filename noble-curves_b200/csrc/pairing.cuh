@@ -23,12 +23,11 @@
 // those of oracle/bls_pairing_ref.py with the same m.
 //
 // A pair with an identity point (the affine (0, 0) encoding) contributes 1; the reference's pairing throws on it.
-// Bodies are host/device so tests/hostemu can run them; the *_serial statements are what the kernels compute.
+// Bodies are host/device so tests/hostemu can run them; the *_serial statements are what the kernels compute.  The
+// check bodies shared with bn254 are pairing_check.cuh's, instantiated with BlsPairing.
 #pragma once
 #include "codec.cuh"
-#include "fp12.cuh"
-#include "msm_body.cuh"
-#include "validate.cuh"
+#include "pairing_check.cuh"
 
 namespace nmsm {
 
@@ -112,50 +111,15 @@ NMSM_HD_NOINLINE BlsF12 bls_final_exp(const BlsF12& f) {
   return fp12_mul(fp12_mul(d, fp12_frobenius<1>(c)), fp12_mul(fp12_frobenius<2>(b), fp12_frobenius<3>(a)));
 }
 
-NMSM_HD bool words_zero(const uint32_t* w, int n) {
-  uint32_t t = 0;
-  for (int k = 0; k < n; k++) t |= w[k];
-  return t == 0;
-}
-
-// k_bls_miller, pair i: validates both points (err[0] = smallest bad G1 index, err[1] = smallest bad G2 index) and
-// writes f_i to out (BLS_F12_WORDS words); rejected and identity pairs write 1.
-NMSM_HD void bls_miller_body(uint64_t i, const uint32_t* g1, const uint32_t* g2, uint32_t* out, unsigned int* err) {
-  uint32_t p[24], q[48];
-  load_words<24>(p, g1 + i * 24);
-  load_words<48>(q, g2 + i * 48);
-  const bool ok1 = point_on_curve<CurveBls381G1Any>(p), ok2 = point_on_curve<CurveBls381G2Any>(q);
-  if (!ok1) atomic_min_u32(&err[0], (uint32_t)i);
-  if (!ok2) atomic_min_u32(&err[1], (uint32_t)i);
-  BlsF12 f = BlsF12::one();
-  if (ok1 && ok2 && !words_zero(p, 24) && !words_zero(q, 48)) f = bls_miller_loop(p, q);
-  f.store(out);
-}
-
-// pairs of check j: [off[j], off[j+1]); off == nullptr means two pairs per check (verification)
-NMSM_HD uint64_t bls_pair_off(const uint64_t* off, uint64_t j) { return off ? off[j] : 2 * j; }
-
-// k_bls_final, check j, over the pair chunk [q0, q1) whose Miller values are W[0 .. q1 - q0).  A check that began in an
-// earlier chunk multiplies in carry_in; one that continues past q1 leaves its partial product in carry_out and no
-// verdict.  Empty checks are skipped (the caller pre-sets their verdict to 1).  pre_ok (optional) is ANDed in.
-NMSM_HD void bls_final_body(uint64_t j, const uint64_t* off, uint64_t q0, uint64_t q1, const uint32_t* W,
-                            const uint32_t* carry_in, uint32_t* carry_out, const uint8_t* pre_ok, uint8_t* out_ok) {
-  const uint64_t a = bls_pair_off(off, j), b = bls_pair_off(off, j + 1);
-  if (a == b) return;
-  BlsF12 f = BlsF12::one(), g;
-  if (a < q0) f.load(carry_in);
-  const uint64_t lo = a < q0 ? q0 : a, hi = b < q1 ? b : q1;
-  for (uint64_t q = lo; q < hi; q++) {
-    g.load(W + (q - q0) * BLS_F12_WORDS);
-    f = fp12_mul(f, g);
-  }
-  if (b > q1) {
-    f.store(carry_out);
-    return;
-  }
-  const bool ok = bls_final_exp(f).is_one() && (!pre_ok || pre_ok[j]);
-  out_ok[j] = ok ? 1 : 0;
-}
+// the pairing policy of pairing_check.cuh
+struct BlsPairing {
+  using F12 = BlsF12;
+  static constexpr int G1_WORDS = 24, G2_WORDS = 48;
+  using G1Curve = CurveBls381G1Any;
+  using G2Curve = CurveBls381G2Any;
+  NMSM_HD static F12 miller_loop(const uint32_t* p, const uint32_t* q) { return bls_miller_loop(p, q); }
+  NMSM_HD static F12 final_exp(const F12& f) { return bls_final_exp(f); }
+};
 
 // the generator of G1, negated: (Gx, p - Gy) canonical
 NMSM_HD uint32_t bls_neg_g1(int k) {
@@ -210,22 +174,11 @@ NMSM_HD void bls_verify_prepare_body(uint32_t i, const uint8_t* sigs96, const ui
   pre_ok[i] = ok ? 1 : 0;
 }
 
-// ---- serial statements (tests/hostemu): the kernels' work for pairs/checks in order, with chunks of `chunk` pairs ----
+// ---- serial statement (tests/hostemu): the kernels' work for pairs/checks in order, with chunks of `chunk` pairs ----
 // W: (chunk + 2) * BLS_F12_WORDS words (the Miller values and two carry slots, as the library's workspace)
 NMSM_HD void bls_check_serial(uint64_t n_checks, const uint64_t* off, const uint32_t* g1, const uint32_t* g2,
                               const uint8_t* pre_ok, uint64_t chunk, uint32_t* W, uint8_t* out_ok, unsigned int* err) {
-  const uint64_t total = bls_pair_off(off, n_checks);
-  for (uint64_t j = 0; j < n_checks; j++) out_ok[j] = 1;
-  uint64_t c = 0;
-  for (uint64_t q0 = 0; q0 < total; q0 += chunk, c++) {
-    const uint64_t q1 = q0 + chunk < total ? q0 + chunk : total;
-    for (uint64_t q = q0; q < q1; q++) bls_miller_body(q, g1, g2, W + (q - q0) * BLS_F12_WORDS, err);
-    uint32_t* carry_in = W + (chunk + ((c + 1) & 1)) * BLS_F12_WORDS;
-    uint32_t* carry_out = W + (chunk + (c & 1)) * BLS_F12_WORDS;
-    for (uint64_t j = 0; j < n_checks; j++)
-      if (bls_pair_off(off, j + 1) > q0 && bls_pair_off(off, j) < q1)
-        bls_final_body(j, off, q0, q1, W, carry_in, carry_out, pre_ok, out_ok);
-  }
+  pairing_check_serial<BlsPairing>(n_checks, off, g1, g2, pre_ok, chunk, W, out_ok, err);
 }
 
 }  // namespace nmsm

@@ -998,25 +998,44 @@ def _bls_g2_compress(pt) -> bytes:
     return bytes(b)
 
 
+def _pack_pairing_checks(checks, G1, G2, label: str):
+    """lists of (G1 Point, G2 Point) pairs -> the packed arguments of a pairing-check entry point"""
+    import struct
+
+    g1, g2, offs = [], [], [0]
+    for j, check in enumerate(checks):
+        for pair in check:
+            if len(pair) != 2 or not isinstance(pair[0], G1) or not isinstance(pair[1], G2):
+                raise TypeError("check %d: (%s.G1.Point, %s.G2.Point) pairs expected" % (j, label, label))
+            g1.append(pair[0])
+            g2.append(pair[1])
+        offs.append(len(g1))
+    return _pack_points(g1), _pack_points(g2), struct.pack("<%dQ" % len(offs), *offs), len(checks)
+
+
+def _pairing_check_call(fn: str, g1_bytes: int, g1_xy: bytes, g2_xy: bytes, pair_off: bytes, n_checks: int) -> bytes:
+    """the C call of a pairing-check entry point fn with G1 points of g1_bytes bytes (G2 points are twice that)"""
+    if len(pair_off) != 8 * (n_checks + 1):
+        raise ValueError("packed arrays do not match n_checks")
+    total = int.from_bytes(pair_off[-8:], "little") if n_checks else 0
+    if len(g1_xy) != g1_bytes * total or len(g2_xy) != 2 * g1_bytes * total:
+        raise ValueError("packed arrays do not match the pair count")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n_checks, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    _lib.check(getattr(lib, fn)(cp(g1_xy or b"\0"), cp(g2_xy or b"\0"), cp(pair_off), n_checks, out))
+    return out.raw[:n_checks]
+
+
 def pairing_check_batch(checks) -> List[bool]:
     """One verdict per check: checks[j] is a list of (G1 Point, G2 Point) pairs, True iff the product of their pairings
     is 1 (noble's pairingBatch compared with Fp12.ONE).  A pair with an identity point contributes 1 (the reference
     throws on the zero point); points are not subgroup-checked (assertValidity / isTorsionFree does that).  Raises
     ValueError for a point off its curve."""
-    G1, G2 = bls12_381.G1.Point, bls12_381.G2.Point
-    g1, g2, offs = [], [], [0]
-    for j, check in enumerate(checks):
-        for pair in check:
-            if len(pair) != 2 or not isinstance(pair[0], G1) or not isinstance(pair[1], G2):
-                raise TypeError("check %d: (bls12_381.G1.Point, bls12_381.G2.Point) pairs expected" % j)
-            g1.append(pair[0])
-            g2.append(pair[1])
-        offs.append(len(g1))
-    import struct
-
+    args = _pack_pairing_checks(checks, bls12_381.G1.Point, bls12_381.G2.Point, "bls12_381")
     try:
-        out = pairing_check_batch_packed(_pack_points(g1), _pack_points(g2), struct.pack("<%dQ" % len(offs), *offs),
-                                         len(checks))
+        out = pairing_check_batch_packed(*args)
     except NmsmError as e:
         _raise_mapped(e)
     return [b == 1 for b in out]
@@ -1026,18 +1045,7 @@ def pairing_check_batch_packed(g1_xy: bytes, g2_xy: bytes, pair_off: bytes, n_ch
     """The C-ABI call itself (nmsm_bls12_381_pairing_check_batch): packed affine G1 (96 B) and G2 (192 B) points and
     n_checks + 1 little-endian u64 pair offsets.  Returns n_checks verdict bytes; raises NmsmError (with .code and
     .index) on an error."""
-    if len(pair_off) != 8 * (n_checks + 1):
-        raise ValueError("packed arrays do not match n_checks")
-    total = int.from_bytes(pair_off[-8:], "little") if n_checks else 0
-    if len(g1_xy) != 96 * total or len(g2_xy) != 192 * total:
-        raise ValueError("packed arrays do not match the pair count")
-    _lib.ensure_init()
-    lib = _lib.load()
-    out = ctypes.create_string_buffer(max(n_checks, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    _lib.check(lib.nmsm_bls12_381_pairing_check_batch(cp(g1_xy or b"\0"), cp(g2_xy or b"\0"), cp(pair_off), n_checks,
-                                                      out))
-    return out.raw[:n_checks]
+    return _pairing_check_call("nmsm_bls12_381_pairing_check_batch", 96, g1_xy, g2_xy, pair_off, n_checks)
 
 
 def bls_verify_batch(signatures, message_points, public_keys) -> List[bool]:
@@ -1099,6 +1107,70 @@ def _bls_verify(signature, message, publicKey) -> bool:
 
 
 bls12_381.verify = _bls_verify
+
+
+# ---- bn254 pairing checks (include/nmsm.h nmsm_bn254_pairing_check_batch) and EIP-197 ecPairing ---------------------
+def bn254_pairing_check_batch(checks) -> List[bool]:
+    """pairing_check_batch on bn254: checks[j] is a list of (bn254.G1.Point, bn254.G2.Point) pairs, True iff the
+    product of their pairings is 1 (noble's bn254.pairingBatch compared with Fp12.ONE).  A pair with an identity point
+    contributes 1; points are not subgroup-checked.  Raises ValueError for a point off its curve."""
+    args = _pack_pairing_checks(checks, bn254.G1.Point, bn254.G2.Point, "bn254")
+    try:
+        out = bn254_pairing_check_batch_packed(*args)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return [b == 1 for b in out]
+
+
+def bn254_pairing_check_batch_packed(g1_xy: bytes, g2_xy: bytes, pair_off: bytes, n_checks: int) -> bytes:
+    """The C-ABI call itself (nmsm_bn254_pairing_check_batch): packed affine G1 (64 B) and G2 (128 B) points and
+    n_checks + 1 little-endian u64 pair offsets.  Returns n_checks verdict bytes; raises NmsmError (with .code and
+    .index) on an error."""
+    return _pairing_check_call("nmsm_bn254_pairing_check_batch", 64, g1_xy, g2_xy, pair_off, n_checks)
+
+
+def bn254_eip197_pairing_batch(inputs) -> List[bool]:
+    """Ethereum's ecPairing precompile (EIP-197) over a batch: one input byte string per call, one verdict per input.
+    An input is k x 192 bytes, per pair G1 x, y then G2 x_imag, x_real, y_imag, y_real, each 32 B big-endian; an
+    all-zero point is the identity; an empty input is True.  Everything the precompile rejects raises ValueError naming
+    the input: a length that is not a multiple of 192, a coordinate >= p, a point off its curve, a G2 point outside the
+    subgroup (nmsm_points_torsion_free)."""
+    import struct
+
+    inputs = list(inputs)
+    if not inputs:
+        return []
+    g1, g2, offs, owner = [], [], [0], []
+    for j, data in enumerate(inputs):
+        if not isinstance(data, (bytes, bytearray, memoryview)):
+            raise TypeError("input %d: bytes expected, got type=%s" % (j, type(data).__name__))
+        data = bytes(data)
+        if len(data) % 192:
+            raise ValueError("input %d: length %d is not a multiple of 192" % (j, len(data)))
+        for k in range(0, len(data), 192):
+            c = [int.from_bytes(data[k + 32 * i:k + 32 * i + 32], "big") for i in range(6)]
+            if any(v >= _BN_P for v in c):
+                raise ValueError("input %d: pair %d has a coordinate >= p" % (j, k // 192))
+            g1.append(c[0].to_bytes(32, "little") + c[1].to_bytes(32, "little"))
+            g2.append(b"".join(c[i].to_bytes(32, "little") for i in (3, 2, 5, 4)))
+            owner.append(j)
+        offs.append(len(g1))
+    n = len(owner)
+    g1_xy, g2_xy = b"".join(g1), b"".join(g2)
+    if n:
+        for what, cid, pts in (("G1", BN254_G1, g1_xy), ("G2", BN254_G2, g2_xy)):
+            bad = points_on_curve(cid, pts, n).find(b"\0")
+            if bad >= 0:
+                raise ValueError("input %d: %s point of pair %d is not on the curve"
+                                 % (owner[bad], what, bad - offs[owner[bad]]))
+        bad = torsion_free_packed(BN254_G2, g2_xy, n).find(b"\0")
+        if bad >= 0:
+            raise ValueError("input %d: G2 point of pair %d is not in the subgroup" % (owner[bad], bad - offs[owner[bad]]))
+    try:
+        out = bn254_pairing_check_batch_packed(g1_xy, g2_xy, struct.pack("<%dQ" % len(offs), *offs), len(inputs))
+    except NmsmError as e:
+        _raise_mapped(e)
+    return [b == 1 for b in out]
 
 
 DECODE_ZIP215 = 1  # include/nmsm.h NMSM_DECODE_ZIP215
