@@ -158,6 +158,58 @@ def hostemu():
     return _emu
 
 
+# ------------------------------------------------------------------------------------------
+# device arithmetic harness (tests/devemu): the device headers' parts compiled for sm_90a and run one case per thread
+# ------------------------------------------------------------------------------------------
+_dev = None
+# (source, object, extra flags): the field unit once with the product's out-of-line multiplications and once inlined
+# (the Makefile's `make EXTRA=` build), whose entry points end in _inl
+DEVEMU_UNITS = [("field.cu", "field.o", ["-DNMSM_MUL_NOINLINE"]), ("field.cu", "field_inl.o", []),
+                ("tower.cu", "tower.o", ["-DNMSM_MUL_NOINLINE"]), ("group.cu", "group.o", ["-DNMSM_MUL_NOINLINE"])]
+
+
+def _nvcc():
+    import shutil
+
+    return shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
+
+
+def devemu():
+    """ctypes handle of tests/devemu/libdevemu.so, (re)built with nvcc for sm_90a when a source or header is newer.  The
+    translation units compile in parallel; ptxas reports (-Xptxas -v) go to tests/devemu/build/*.log."""
+    global _dev
+    if _dev is not None:
+        return _dev
+    d = os.path.join(ROOT, "tests", "devemu")
+    so = os.path.join(d, "libdevemu.so")
+    csrc = os.path.join(ROOT, "noble-curves_b200", "csrc")
+    deps = [os.path.join(d, f) for f in os.listdir(d) if f.endswith((".cu", ".cuh"))]
+    deps += [os.path.join(csrc, f) for f in os.listdir(csrc) if f.endswith((".cuh", ".h"))]
+    if not os.path.exists(so) or any(os.path.getmtime(x) > os.path.getmtime(so) for x in deps):
+        bdir = os.path.join(d, "build")
+        os.makedirs(bdir, exist_ok=True)
+        nvcc = _nvcc()
+        flags = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v",
+                 "-I", csrc]
+        procs = []
+        for src, obj, extra in DEVEMU_UNITS:
+            log = open(os.path.join(bdir, obj[:-2] + ".log"), "w")
+            cmd = [nvcc] + flags + extra + ["-c", os.path.join(d, src), "-o", os.path.join(bdir, obj)]
+            procs.append((subprocess.Popen(cmd, stdout=log, stderr=subprocess.STDOUT), log, obj))
+        failed = []
+        for proc, log, obj in procs:
+            if proc.wait() != 0:
+                failed.append(obj)
+            log.close()
+        if failed:
+            msgs = [open(os.path.join(bdir, o[:-2] + ".log")).read()[-4000:] for o in failed]
+            raise RuntimeError("devemu build failed: %s\n%s" % (failed, "\n".join(msgs)))
+        subprocess.check_call([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", so]
+                              + [os.path.join(bdir, obj) for _, obj, _ in DEVEMU_UNITS])
+    _dev = ctypes.CDLL(so)
+    return _dev
+
+
 def u32(b: bytes):
     return np.frombuffer(b, dtype=np.uint32).copy()
 

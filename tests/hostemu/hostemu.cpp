@@ -310,9 +310,18 @@ static void field_op(int op, const uint32_t* a, const uint32_t* b, uint32_t* r) 
     case 6: z = sqr(x); break;
     case 8: z = DivstepsInv<P>::inverse(x); break;                                  // Montgomery in / out
     case 9: if (!DivstepsInv<P>::inverse_words(a, z.v)) z = Fp<P>::zero(); break;    // plain integers
+    case 11: z = Fp<P>::zero(); z.v[0] = Fp<P>::canonical_in_range(a) ? 1u : 0u; break;
     default: z = -x; break;
   }
   for (int i = 0; i < P::N; i++) r[i] = z.v[i];
+}
+
+// op 0: T = a * b as 2N words (any N-limb a, b); op 1: T / R mod p of a 2N-word T < p R / 2 (field.cuh mul_wide,
+// mont_reduce_wide)
+template <class P>
+static void wide_op(int op, const uint32_t* a, const uint32_t* b, uint32_t* r) {
+  if (op == 0) mul_wide<P>(r, a, b);
+  else mont_reduce_wide<P>(r, a);
 }
 
 static int emu_ed_verify(const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs, const uint64_t* off, uint32_t n,
@@ -337,8 +346,9 @@ static int emu_ed_verify(const uint8_t* sigs, const uint8_t* pks, const uint8_t*
   return 0;
 }
 
-// Fp2 product of Montgomery-form operands (a, b, r: c0 limbs then c1 limbs), both statements of the multiplication:
-// form 0 = three reduced base multiplications (tower.ts:420-431 order), form 1 = Karatsuba with lazy reduction
+// Fp2 operations on Montgomery-form operands (a, b, r: c0 limbs then c1 limbs), both statements of the multiplication:
+// form 0 = three reduced base multiplications (tower.ts:420-431 order), form 1 = Karatsuba with lazy reduction,
+// form 2 = operator*, form 3 = sqr, form 4 = inv
 template <class P>
 static void fp2_mul_forms(int form, const uint32_t* a, const uint32_t* b, uint32_t* r) {
   Fp2<P> x, y, z;
@@ -348,6 +358,12 @@ static void fp2_mul_forms(int form, const uint32_t* a, const uint32_t* b, uint32
   }
   if (form == 1) {
     z = Fp2<P>::mul_lazy(x, y);
+  } else if (form == 2) {
+    z = x * y;
+  } else if (form == 3) {
+    z = sqr(x);
+  } else if (form == 4) {
+    z = inv(x);
   } else {
     Fp<P> t1 = x.c0 * y.c0, t2 = x.c1 * y.c1;
     z = Fp2<P>{t1 - t2, (x.c0 + x.c1) * (y.c0 + y.c1) - (t1 + t2)};
@@ -454,14 +470,41 @@ int emu_fp2_mul(int field, int form, const uint32_t* a, const uint32_t* b, uint3
   if (field == 3) { fp2_mul_forms<FpBls381>(form, a, b, r); return 0; }
   return -1;
 }
-// field: 0 secp256k1, 1 ed25519, 2 bn254, 3 bls12-381
+// field: 0 secp256k1 p, 1 ed25519 p, 2 bn254 p, 3 bls12-381 p, 4 secp256k1 n, 5 ed25519 l, 6 bn254 r, 7 bls12-381 r
 int emu_field(int field, int op, const uint32_t* a, const uint32_t* b, uint32_t* r) {
   switch (field) {
     case 0: field_op<FpSecp256k1>(op, a, b, r); return 0;
     case 1: field_op<FpEd25519>(op, a, b, r); return 0;
     case 2: field_op<FpBn254>(op, a, b, r); return 0;
     case 3: field_op<FpBls381>(op, a, b, r); return 0;
+    case 4: field_op<FnSecp256k1Mod>(op, a, b, r); return 0;
+    case 5: field_op<FnEd25519Mod>(op, a, b, r); return 0;
+    case 6: field_op<FrBn254>(op, a, b, r); return 0;
+    case 7: field_op<FrBls381>(op, a, b, r); return 0;
   }
   return -1;
+}
+// batched forms of emu_field / field_op, wide_op and emu_fp2_mul: n cases laid out back to back, the interface of
+// tests/devemu's dev_field / dev_wide / dev_fp2
+int emu_field_n(int field, int op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* r) {
+  if (field < 0 || field > 7) return -1;
+  const size_t N = field == 3 ? 12 : 8;
+  for (uint32_t i = 0; i < n; i++) emu_field(field, op, a + i * N, b + i * N, r + i * N);
+  return 0;
+}
+int emu_wide_n(int field, int op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* r) {
+  if (field != 2 && field != 3) return -1;
+  const size_t N = field == 3 ? 12 : 8, wa = op == 0 ? N : 2 * N, wr = op == 0 ? 2 * N : N;
+  for (uint32_t i = 0; i < n; i++) {
+    if (field == 2) wide_op<FpBn254>(op, a + i * wa, b + i * N, r + i * wr);
+    else wide_op<FpBls381>(op, a + i * wa, b + i * N, r + i * wr);
+  }
+  return 0;
+}
+int emu_fp2_n(int field, int form, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* r) {
+  if (field != 2 && field != 3) return -1;
+  const size_t W = field == 3 ? 24 : 16;
+  for (uint32_t i = 0; i < n; i++) emu_fp2_mul(field, form, a + i * W, b + i * W, r + i * W);
+  return 0;
 }
 }

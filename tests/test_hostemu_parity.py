@@ -10,77 +10,78 @@ import random
 
 import pytest
 
+import arith_cases as A
 import helpers as H
 from oracle import noble_ref as R
 
 ALL = ["secp256k1", "ed25519", "bn254_G1", "bn254_G2", "bls12_381_G1", "bls12_381_G2"]
-FIELDS = {
-    0: R.SECP256K1_CURVE["p"],
-    1: R.ED25519_CURVE["p"],
-    2: R.BN254_G1_CURVE["p"],
-    3: R.BLS12_381_G1_CURVE["p"],
-}
+FIELDS = {fid: p for fid, (_, p, _) in A.FIELDS.items()}
 
 
 def _fop(field, op, a, b=0):
+    return _fop_n(field, op, [a], [b])[0]
+
+
+def _fop_n(field, op, avals, bvals=None):
+    """emu_field_n over a batch: Montgomery / plain words in, ints out"""
     import ctypes
 
     import numpy as np
 
-    p = FIELDS[field]
-    n = 12 if field == 3 else 8
-    la = H.u32(a.to_bytes(4 * n, "little"))
-    lb = H.u32(b.to_bytes(4 * n, "little"))
-    out = np.zeros(n, np.uint32)
+    n = A.FIELDS[field][2]
+    la = np.array(A.words(avals, n), np.uint32)
+    lb = np.array(A.words(bvals if bvals is not None else [0] * len(avals), n), np.uint32)
+    out = np.zeros(len(avals) * n, np.uint32)
     cp = lambda x: x.ctypes.data_as(ctypes.c_void_p)  # noqa: E731
-    assert H.hostemu().emu_field(field, op, cp(la), cp(lb), cp(out)) == 0
-    return int.from_bytes(out.tobytes(), "little")
+    assert H.hostemu().emu_field_n(field, op, len(avals), cp(la), cp(lb), cp(out)) == 0
+    return A.ints(out, n)
 
 
-@pytest.mark.parametrize("field", [0, 1, 2, 3])
+def _label(field, op):
+    return "%s op %d" % (A.FIELDS[field][0], op)
+
+
+@pytest.mark.parametrize("field", sorted(A.FIELDS))
 def test_field_ops_match_bigint(field):
-    """mont_mul/add/sub/neg/sqr/inv/from/to-Montgomery vs Python ints (modular.ts:888-1038 semantics)."""
-    p = FIELDS[field]
-    n = 12 if field == 3 else 8
+    """mont_mul/add/sub/neg/sqr/inv/from/to-Montgomery/canonical_in_range vs Python ints (modular.ts:888-1038 semantics),
+    for the four base fields and the four scalar fields, on arith_cases' carry-edge values and Montgomery-target pairs."""
+    _, p, n = A.FIELDS[field]
     Rm = 1 << (32 * n)
     Ri = pow(Rm, -1, p)
-    rnd = random.Random(1234 + field)
-    edge = [0, 1, 2, p - 1, p - 2, Rm % p, (Rm * Rm) % p, p >> 1, (1 << (p.bit_length() - 1)) % p]
-    vals = edge + [rnd.randrange(p) for _ in range(60)]
-    for a in vals:
-        for b in rnd.sample(vals, 6) + edge[:4]:
-            assert _fop(field, 0, a, b) == (a * b * Ri) % p
-            assert _fop(field, 1, a, b) == (a + b) % p
-            assert _fop(field, 2, a, b) == (a - b) % p
-        assert _fop(field, 6, a) == (a * a * Ri) % p
-        assert _fop(field, 7, a) == (-a) % p
-        assert _fop(field, 4, a) == (a * Rm) % p  # from_canonical
-        assert _fop(field, 5, (a * Rm) % p) == a  # to_canonical
-    for a in vals[:12]:
-        exp = (pow(a, -1, p) * Rm) % p if a else 0
-        assert _fop(field, 3, (a * Rm) % p) == exp
+    pairs = A.binary_pairs(field)
+    a = [x for x, _ in pairs]
+    b = [y for _, y in pairs]
+    A.assert_same(_label(field, A.MUL), _fop_n(field, A.MUL, a, b), [x * y * Ri % p for x, y in pairs], pairs)
+    A.assert_same(_label(field, A.ADD), _fop_n(field, A.ADD, a, b), [(x + y) % p for x, y in pairs], pairs)
+    A.assert_same(_label(field, A.SUB), _fop_n(field, A.SUB, a, b), [(x - y) % p for x, y in pairs], pairs)
+    vals = A.field_values(field)
+    A.assert_same(_label(field, A.SQR), _fop_n(field, A.SQR, vals), [x * x * Ri % p for x in vals], vals)
+    A.assert_same(_label(field, A.NEG), _fop_n(field, A.NEG, vals), [(-x) % p for x in vals], vals)
+    A.assert_same(_label(field, A.FROM_MONT_IN), _fop_n(field, A.FROM_MONT_IN, vals), [x * Rm % p for x in vals], vals)
+    mont = [x * Rm % p for x in vals]
+    A.assert_same(_label(field, A.TO_CANON), _fop_n(field, A.TO_CANON, mont), vals, mont)
+    near = vals + [p, p + 1, 2 * p - 1 if 2 * p < Rm else p + 2, Rm - 1, p | 0xFFFFFFFF, p + (1 << 32)]
+    near = [x for x in near if x < Rm]
+    A.assert_same(_label(field, A.IN_RANGE), [w & 1 for w in _fop_n(field, A.IN_RANGE, near)],
+                  [1 if x < p else 0 for x in near], near)
+    inv_in = mont[:16]
+    A.assert_same(_label(field, A.INV_XGCD), _fop_n(field, A.INV_XGCD, inv_in),
+                  [(pow(x, -1, p) * Rm) % p if x else 0 for x in vals[:16]], inv_in)
 
 
-@pytest.mark.parametrize("field", [0, 1, 2, 3])
+@pytest.mark.parametrize("field", sorted(A.FIELDS))
 def test_divsteps_inverse(field):
-    """csrc/inv_divsteps.cuh (experimental, not yet used by the kernels): batched division-step inversion equals
-    pow(x, -1, p) on plain integers and equals field.cuh's inv in Montgomery form, on edge values and random ones."""
-    import random as _r
-
-    p = FIELDS[field]
-    n = 12 if field == 3 else 8
+    """csrc/inv_divsteps.cuh: batched division-step inversion equals pow(x, -1, p) on plain integers and equals
+    field.cuh's inv in Montgomery form, for all eight moduli, on arith_cases' edge values and random ones."""
+    _, p, n = A.FIELDS[field]
     Rm = pow(2, 32 * n, p)
-    rnd = _r.Random(field)
-    vals = [1, 2, 3, p - 1, p - 2, (p + 1) // 2, (p - 1) // 2, 1 << 30, (1 << 30) - 1, 1 << 60, (1 << 255) % p,
-            (1 << (p.bit_length() - 1)) - 1, 0x55555555555555555555555555555555 % p, pow(3, 200, p)]
-    vals += [rnd.randrange(1, p) for _ in range(300)]
-    vals += [rnd.randrange(1, 1 << k) for k in (8, 31, 61, 64, 90, 200) for _ in range(5)]
-    for x in vals:
-        assert _fop(field, 9, x) == pow(x, -1, p), hex(x)
-    for x in vals[:60]:
-        xm = x * Rm % p
-        assert _fop(field, 8, xm) == _fop(field, 3, xm) == _fop(field, 10, xm) == pow(x, -1, p) * Rm % p
-    assert _fop(field, 8, 0) == 0
+    vals = A.inverse_values(field)
+    A.assert_same(_label(field, A.INV_WORDS), _fop_n(field, A.INV_WORDS, vals), [pow(x, -1, p) for x in vals], vals)
+    xm = [x * Rm % p for x in vals[:60]]
+    want = [pow(x, -1, p) * Rm % p for x in vals[:60]]
+    for op in (A.DIVSTEPS, A.INV_XGCD, A.INV):
+        A.assert_same(_label(field, op), _fop_n(field, op, xm), want, xm)
+    assert _fop(field, A.DIVSTEPS, 0) == 0
 
 
 @pytest.mark.parametrize("field", [2, 3])
