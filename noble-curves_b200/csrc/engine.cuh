@@ -73,6 +73,8 @@ static bool prepare_on_side_stream(uint64_t n, bool prepared) { return !g_ctx.pr
 // H2D of host inputs: scalars first on the main stream (the digit passes only need them), the 3x larger point array on
 // prep_stream where k_prepare follows it — the digit count / scan / scatter overlap the point copy.
 static int stage_host_inputs(Slot& C, const void* pts, const void* scalars, uint64_t n) {
+  // submit_msm's bound, checked here before n-sized buffers are allocated and filled (else: an out-of-memory error)
+  if (n >= (1ull << 31)) return fail(NMSM_ERR_ARG, "n must be < 2^31");
   CK(C.in_pts.ensure(n * G::IN_WORDS * 4));
   CK(C.in_scalars.ensure(n * SCALAR_WORDS * 4));
   // h2d_any: pinned sources are one DMA each; large pageable ones are staged through pinned chunks by worker threads
