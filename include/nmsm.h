@@ -23,6 +23,8 @@
  *   nmsm_ed25519_verify_batch <- ed25519.verify over a batch      edwards.ts:942-989
  *   nmsm_secp256k1_verify_batch <- secp256k1.verify over a batch, one verdict per signature (weierstrass.ts ecdsa().verify)
  *   nmsm_secp256k1_schnorr_verify_batch <- schnorr.verify over a batch, one verdict per signature (secp256k1.ts, BIP340)
+ *   nmsm_secp256k1_recover_batch <- secp256k1.recoverPublicKey over a batch (weierstrass.ts Signature.recoverPublicKey)
+ *   nmsm_secp256k1_ecrecover_batch <- Ethereum's ecrecover precompile (0x01) over a batch
  *   nmsm_bls12_381_pairing_check_batch / nmsm_bn254_pairing_check_batch <- pairingBatch(...) == 1, one verdict per check
  *   nmsm_ntt           <- FFT(rootsOfUnity(Fr, G), Fr).direct / .inverse   src/abstract/fft.ts:518-575
  *
@@ -238,6 +240,32 @@ int nmsm_secp256k1_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, con
  * nmsm_last_timing reports k_schnorr_prepare in slot 0, k_schnorr_check in slot 1 and both in NMSM_T_TOTAL. */
 int nmsm_secp256k1_schnorr_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint8_t* msgs,
                                         const uint64_t* msg_off, uint64_t n, uint8_t* out_ok);
+
+/* secp256k1 ECDSA public-key recovery (next-row f9): the batch form of noble-curves v2
+ * secp256k1.recoverPublicKey(signature, message, { prehash }) with the 65-byte 'recovered' signature format.
+ * sigs65: n x 65 B = recovery id (1 B) || r || s (32 B each, big-endian).  message i = msgs[msg_off[i], msg_off[i+1]).
+ * flags: 0 or NMSM_ECDSA_PREHASH.  out_xy: n x 64 B, the recovered key in the library's affine packing (little-endian
+ * x || y, as nmsm_mul_batch writes it); out_ok: n bytes, 1 = recovered.  A failed item gets out_ok 0 and 64 zero
+ * bytes, never an error.  The rules (weierstrass.ts Signature.recoverPublicKey; each failure is where it throws):
+ *   recovery id rec in {0, 1, 2, 3};  1 <= r < n, 1 <= s < n (no lowS rule: a high s recovers);
+ *   x = r + n if rec & 2, else r;  x < p;  R = the SEC1 decode of (rec & 1 ? 03 : 02) || x (x^3 + 7 must be a square);
+ *   h = bits2int_modN(prehash ? sha256(msg) : msg), a raw message over 8192 bytes fails as in verify;
+ *   u1 = -h r^-1, u2 = s r^-1 (mod n);  Q = u1 G + u2 R;  Q = O fails.
+ * NMSM_ERR_ARG is for null pointers, offsets that do not start at 0 or decrease, unknown flag bits and n >= 2^31.  n == 0
+ * writes nothing.  Shares the fixed-point table of G with the ECDSA and Schnorr verifiers and
+ * nmsm_secp256k1_ecrecover_batch: whichever of the four runs first after nmsm_init builds it.  With profiling on,
+ * nmsm_last_timing reports k_recover_prepare in slot 0, k_recover_check in slot 1 and both in NMSM_T_TOTAL. */
+int nmsm_secp256k1_recover_batch(const uint8_t* sigs65, const uint8_t* msgs, const uint64_t* msg_off, uint64_t n,
+                                 int flags, uint8_t* out_xy, uint8_t* out_ok);
+
+/* Ethereum ecrecover (precompile 0x01, Yellow Paper appendix E), batched.  inputs128: n x 128 B = h (32) || v (32,
+ * big-endian integer) || r || s.  v must equal 27 or 28 as a 256-bit integer (bytes 32..62 zero), rec = v - 27;
+ * 1 <= r, s < n with no lowS rule (EIP-2 is a transaction rule, not the precompile's); h is the 32 raw bytes
+ * (bits2int_modN without prehash); then recovery runs as in nmsm_secp256k1_recover_batch.
+ * out32: n x 32 B = 12 zero bytes || the last 20 bytes of keccak256(x_be || y_be) of the recovered key; out_ok: n bytes.
+ * Where the precompile returns empty output: out_ok 0 and 32 zero bytes.  Errors, the table of G and the profiling
+ * slots as for nmsm_secp256k1_recover_batch. */
+int nmsm_secp256k1_ecrecover_batch(const uint8_t* inputs128, uint64_t n, uint8_t* out32, uint8_t* out_ok);
 
 /* BLS12-381 batch pairing checks (next-row f7): out_ok[j] = 1 iff prod_{i in [pair_off[j], pair_off[j+1])} e(P_i, Q_i)
  * == 1 in GT, the optimal-ate pairing of the reference (src/abstract/bls.ts, bls12-381.ts), one verdict per check.

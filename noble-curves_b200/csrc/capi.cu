@@ -768,6 +768,7 @@ int nmsm_secp256k1_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, con
   SLOT0_FREE();
   if (flags & ~(NMSM_ECDSA_PREHASH | NMSM_ECDSA_LOW_S)) return fail(NMSM_ERR_ARG, "nmsm_secp256k1_verify_batch: unknown flag");
   if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 31)) return fail(NMSM_ERR_ARG, "n must be < 2^31");  // before pk_off[n] / msg_off[n] are read
   if (!sigs || !pk_off || !msg_off || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
   if ((pk_off[n] && !pubkeys) || (msg_off[n] && !msgs)) return fail(NMSM_ERR_ARG, "null pointer");
   return secp256k1_verify_batch_impl(sigs, pubkeys, pk_off, msgs, msg_off, n, flags, out_ok);
@@ -780,9 +781,35 @@ int nmsm_secp256k1_schnorr_verify_batch(const uint8_t* sigs, const uint8_t* pubk
   g_ctx.cur = 0;
   SLOT0_FREE();
   if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 31)) return fail(NMSM_ERR_ARG, "n must be < 2^31");  // before msg_off[n] is read
   if (!sigs || !pubkeys || !msg_off || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
   if (msg_off[n] && !msgs) return fail(NMSM_ERR_ARG, "null pointer");
   return secp256k1_schnorr_verify_batch_impl(sigs, pubkeys, msgs, msg_off, n, out_ok);
+}
+
+int nmsm_secp256k1_recover_batch(const uint8_t* sigs65, const uint8_t* msgs, const uint64_t* msg_off, uint64_t n,
+                                 int flags, uint8_t* out_xy, uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (flags & ~NMSM_ECDSA_PREHASH) return fail(NMSM_ERR_ARG, "nmsm_secp256k1_recover_batch: unknown flag");
+  if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 31)) return fail(NMSM_ERR_ARG, "n must be < 2^31");  // before msg_off[n] is read
+  if (!sigs65 || !msg_off || !out_xy || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
+  if (msg_off[n] && !msgs) return fail(NMSM_ERR_ARG, "null pointer");
+  return secp256k1_recover_batch_impl(sigs65, msgs, msg_off, n, flags, out_xy, out_ok);
+}
+
+int nmsm_secp256k1_ecrecover_batch(const uint8_t* inputs128, uint64_t n, uint8_t* out32, uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 31)) return fail(NMSM_ERR_ARG, "n must be < 2^31");
+  if (!inputs128 || !out32 || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
+  return secp256k1_ecrecover_batch_impl(inputs128, n, out32, out_ok);
 }
 
 int nmsm_bls12_381_pairing_check_batch(const uint8_t* g1_xy, const uint8_t* g2_xy, const uint64_t* pair_off,

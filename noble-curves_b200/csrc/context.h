@@ -208,6 +208,9 @@ int secp256k1_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const u
                                 const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
 int secp256k1_schnorr_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs,
                                         const uint64_t* msg_off, uint64_t n, uint8_t* out_ok);
+int secp256k1_recover_batch_impl(const uint8_t* sigs65, const uint8_t* msgs, const uint64_t* msg_off, uint64_t n,
+                                 int flags, uint8_t* out_xy, uint8_t* out_ok);
+int secp256k1_ecrecover_batch_impl(const uint8_t* inputs128, uint64_t n, uint8_t* out32, uint8_t* out_ok);
 int bls12_381_pairing_check_batch_impl(const uint8_t* g1_xy, const uint8_t* g2_xy, const uint64_t* pair_off,
                                        uint64_t n_checks, uint8_t* out_ok);
 int bn254_pairing_check_batch_impl(const uint8_t* g1_xy, const uint8_t* g2_xy, const uint64_t* pair_off,

@@ -121,6 +121,30 @@ NMSM_HD bool ecdsa_high_s(const uint32_t* s) {
   return false;
 }
 
+// h = bits2int_modN(prehash ? sha256(m) : m) for the message m[0..mlen): the big-endian integer of the first
+// min(len, 32) bytes, reduced mod n.  False for a raw message over ECDSA_MAX_RAW_MSG bytes (bits2int throws).
+NMSM_HD bool ecdsa_msg_hash(const uint8_t* m, uint64_t mlen, int flags, uint32_t* h) {
+  uint8_t digest[32];
+  if (flags & ECDSA_PREHASH) {
+    sha256(m, mlen, digest);
+    m = digest;
+    mlen = 32;
+  } else if (mlen > ECDSA_MAX_RAW_MSG) {
+    return false;
+  }
+  const int take = mlen < 32 ? (int)mlen : 32;
+  for (int k = 0; k < 8; k++) h[k] = 0;
+  for (int j = 0; j < take; j++) {
+    const int bit = 8 * (take - 1 - j);
+    h[bit >> 5] |= (uint32_t)m[j] << (bit & 31);
+  }
+  if (!EcS::canonical_in_range(h)) {  // h < 2^256 < 2n: one subtraction reduces it
+    h[0] = sub_cc(h[0], FnSecp256k1Mod::P(0));
+    for (int k = 1; k < 8; k++) h[k] = subc_cc(h[k], FnSecp256k1Mod::P(k));
+  }
+  return true;
+}
+
 // Signature i: r, s, the public key Q (canonical affine words) and h = bits2int_modN(m).  False = the reference's
 // verify returns false before any scalar multiplication; the outputs are then unspecified.
 NMSM_HD bool ecdsa_prepare_body(uint32_t i, const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off,
@@ -142,28 +166,7 @@ NMSM_HD bool ecdsa_prepare_body(uint32_t i, const uint8_t* sigs, const uint8_t* 
   } else {
     return false;
   }
-  // h = bits2int(m) mod n: the big-endian integer of the first min(len, 32) bytes of m
-  const uint8_t* m = msgs + msg_off[i];
-  uint64_t mlen = msg_off[i + 1] - msg_off[i];
-  uint8_t digest[32];
-  if (flags & ECDSA_PREHASH) {
-    sha256(m, mlen, digest);
-    m = digest;
-    mlen = 32;
-  } else if (mlen > ECDSA_MAX_RAW_MSG) {
-    return false;
-  }
-  const int take = mlen < 32 ? (int)mlen : 32;
-  for (int k = 0; k < 8; k++) h[k] = 0;
-  for (int j = 0; j < take; j++) {
-    const int bit = 8 * (take - 1 - j);
-    h[bit >> 5] |= (uint32_t)m[j] << (bit & 31);
-  }
-  if (!EcS::canonical_in_range(h)) {  // h < 2^256 < 2n: one subtraction reduces it
-    h[0] = sub_cc(h[0], FnSecp256k1Mod::P(0));
-    for (int k = 1; k < 8; k++) h[k] = subc_cc(h[k], FnSecp256k1Mod::P(k));
-  }
-  return true;
+  return ecdsa_msg_hash(msgs + msg_off[i], msg_off[i + 1] - msg_off[i], flags, h);
 }
 
 // Given w = s^-1 (Montgomery form mod n): u1 = h w, u2 = r w, and the per-signature state k_ecdsa_check reads.

@@ -17,7 +17,7 @@ argument shapes.  Nothing here imports `oracle/`.
 from __future__ import annotations
 
 import ctypes
-from typing import List, Sequence
+from typing import List, Optional, Sequence
 
 from . import _lib
 from ._lib import NmsmError, PlanInfo, TIMING_NAMES, init  # noqa: F401
@@ -983,6 +983,101 @@ def _schnorr_verify(signature, message, publicKey) -> bool:
 
 
 schnorr = _NS(verify=_schnorr_verify)  # the reference's `schnorr` export (secp256k1.ts)
+
+
+# ---- secp256k1 ECDSA public-key recovery and Ethereum ecrecover (include/nmsm.h nmsm_secp256k1_*recover_batch) -----
+def ecdsa_recover_batch(signatures, messages, prehash: bool = True) -> List[Optional[bytes]]:
+    """Batch form of secp256k1.recoverPublicKey(signature, message, {prehash}) with the 65-byte 'recovered' format
+    rec || r || s (noble-curves weierstrass.ts Signature.recoverPublicKey): per signature the recovered key as 33-byte
+    SEC1 compressed bytes, or None where the reference throws (a recovery id outside 0..3, r or s outside [1, n), an x
+    coordinate >= p or off the curve, a raw message over 8192 bytes, Q = O).  Raises for non-bytes arguments, a
+    signature that is not 65 bytes and lists of different lengths."""
+    n = len(signatures)
+    if len(messages) != n:
+        raise ValueError("signatures and messages must have equal length")
+    for what, items in (("signature", signatures), ("message", messages)):
+        for x in items:
+            if not isinstance(x, (bytes, bytearray, memoryview)):
+                raise TypeError('"%s" expected Uint8Array, got type=%s' % (what, type(x).__name__))
+    for s in signatures:
+        if len(s) != 65:
+            raise ValueError('"recovered signature" expected Uint8Array of length 65, got length=%d' % len(s))
+    xy, ok = ecdsa_recover_batch_packed(b"".join(bytes(s) for s in signatures), b"".join(bytes(m) for m in messages),
+                                        _pack_offsets(messages), n, ECDSA_PREHASH if prehash else 0)
+    out = []
+    for k in range(n):
+        if not ok[k]:
+            out.append(None)
+            continue
+        x, y = xy[64 * k:64 * k + 32], xy[64 * k + 32:64 * k + 64]
+        out.append(bytes([2 + (y[0] & 1)]) + x[::-1])
+    return out
+
+
+def ecdsa_recover_batch_packed(sigs65: bytes, msgs: bytes, msg_off: bytes, n: int, flags: int = ECDSA_PREHASH):
+    """The C-ABI call itself (nmsm_secp256k1_recover_batch) on caller-packed arrays: n*65 signature bytes (rec || r ||
+    s), the concatenated messages with n+1 little-endian u64 offsets.  Returns (n*64 bytes of keys in the affine
+    packing, little-endian x || y, zero for a failed item; n verdict bytes, 1 = recovered)."""
+    if len(sigs65) != 65 * n or len(msg_off) != 8 * (n + 1):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    xy = ctypes.create_string_buffer(max(64 * n, 1))
+    ok = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    rc = lib.nmsm_secp256k1_recover_batch(cp(sigs65 or b"\0"), cp(msgs or b"\0"), cp(msg_off), n, flags, xy, ok)
+    try:
+        _lib.check(rc)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return xy.raw[:64 * n], ok.raw[:n]
+
+
+def _secp256k1_recover_public_key(signature, message, prehash: bool = True) -> bytes:
+    """secp256k1.recoverPublicKey for one signature (the batch entry point with n = 1): the 33-byte compressed key
+    (the reference's default toBytes()).  Raises ValueError where the reference throws."""
+    key = ecdsa_recover_batch([signature], [message], prehash=prehash)[0]
+    if key is None:
+        raise ValueError("public key recovery failed: invalid recovery id, r, s or message, or the key is the point "
+                         "at infinity")
+    return key
+
+
+secp256k1.recoverPublicKey = _secp256k1_recover_public_key
+
+
+def eth_ecrecover_batch(inputs) -> List[bytes]:
+    """Ethereum's ecrecover precompile (0x01) over a batch: per input the precompile's output, the 32-byte word 12
+    zero bytes || address, or b"" where the precompile returns empty output.  An input is right-padded with zeros to
+    128 bytes or truncated to its first 128, as the precompile reads its call data."""
+    inputs = list(inputs)
+    buf = []
+    for j, data in enumerate(inputs):
+        if not isinstance(data, (bytes, bytearray, memoryview)):
+            raise TypeError("input %d: bytes expected, got type=%s" % (j, type(data).__name__))
+        buf.append(bytes(data[:128]).ljust(128, b"\0"))
+    if not buf:
+        return []
+    words, ok = eth_ecrecover_batch_packed(b"".join(buf), len(buf))
+    return [words[32 * k:32 * k + 32] if ok[k] else b"" for k in range(len(buf))]
+
+
+def eth_ecrecover_batch_packed(inputs128: bytes, n: int):
+    """The C-ABI call itself (nmsm_secp256k1_ecrecover_batch): n*128 input bytes h || v || r || s.  Returns (n*32
+    bytes of address words, zero for a failed item; n verdict bytes, 1 = recovered)."""
+    if len(inputs128) != 128 * n:
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    words = ctypes.create_string_buffer(max(32 * n, 1))
+    ok = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    rc = lib.nmsm_secp256k1_ecrecover_batch(cp(inputs128 or b"\0"), n, words, ok)
+    try:
+        _lib.check(rc)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return words.raw[:32 * n], ok.raw[:n]
 
 
 # ---- BLS12-381 pairing checks and BLS signatures (include/nmsm.h nmsm_bls12_381_*) -----------------------------------

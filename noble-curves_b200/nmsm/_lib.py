@@ -41,6 +41,7 @@ EXPORTS = [
     "nmsm_points_decode_ex", "nmsm_points_on_curve", "nmsm_set_window_groups", "nmsm_accs_normalize",
     "nmsm_dist_unique_id", "nmsm_dist_init", "nmsm_dist_info", "nmsm_dist_exchange_mode", "nmsm_msm_sharded", "nmsm_msm_sharded_submit",
     "nmsm_secp256k1_verify_batch", "nmsm_secp256k1_schnorr_verify_batch",
+    "nmsm_secp256k1_recover_batch", "nmsm_secp256k1_ecrecover_batch",
     "nmsm_bls12_381_pairing_check_batch", "nmsm_bls12_381_verify_batch", "nmsm_bn254_pairing_check_batch",
 ]
 
@@ -170,6 +171,10 @@ def load() -> ctypes.CDLL:
         lib.nmsm_secp256k1_verify_batch.restype = ctypes.c_int
         lib.nmsm_secp256k1_schnorr_verify_batch.argtypes = [u8p, u8p, u8p, u8p, ctypes.c_uint64, u8p]
         lib.nmsm_secp256k1_schnorr_verify_batch.restype = ctypes.c_int
+        lib.nmsm_secp256k1_recover_batch.argtypes = [u8p, u8p, u8p, ctypes.c_uint64, ctypes.c_int, u8p, u8p]
+        lib.nmsm_secp256k1_recover_batch.restype = ctypes.c_int
+        lib.nmsm_secp256k1_ecrecover_batch.argtypes = [u8p, ctypes.c_uint64, u8p, u8p]
+        lib.nmsm_secp256k1_ecrecover_batch.restype = ctypes.c_int
         lib.nmsm_bls12_381_pairing_check_batch.argtypes = [u8p, u8p, u8p, ctypes.c_uint64, u8p]
         lib.nmsm_bls12_381_pairing_check_batch.restype = ctypes.c_int
         lib.nmsm_bn254_pairing_check_batch.argtypes = [u8p, u8p, u8p, ctypes.c_uint64, u8p]
