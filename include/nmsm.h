@@ -26,6 +26,8 @@
  *   nmsm_secp256k1_recover_batch <- secp256k1.recoverPublicKey over a batch (weierstrass.ts Signature.recoverPublicKey)
  *   nmsm_secp256k1_ecrecover_batch <- Ethereum's ecrecover precompile (0x01) over a batch
  *   nmsm_bls12_381_pairing_check_batch / nmsm_bn254_pairing_check_batch <- pairingBatch(...) == 1, one verdict per check
+ *   nmsm_bls12_381_hash_to_g2_batch <- bls12_381.G2.hashToCurve(msg, { DST }) over a batch (RFC 9380)
+ *   nmsm_bls12_381_verify_msg_batch <- bls12_381.verify over a batch with the messages hashed on the GPU
  *   nmsm_ntt           <- FFT(rootsOfUnity(Fr, G), Fr).direct / .inverse   src/abstract/fft.ts:518-575
  *
  * Data formats (all little-endian, plain bytes, caller-owned):
@@ -299,7 +301,8 @@ int nmsm_bn254_pairing_check_batch(const uint8_t* g1_xy, const uint8_t* g2_xy, c
 /* BLS12-381 batch signature verification (next-row f7): out_ok[i] = bls12_381.verify(sig_i, H_i, pk_i) for long
  * signatures (public key in G1, signature in G2), one independent verdict per signature.
  * sigs96: n x 96 B Zcash-flag compressed G2 signatures; pks48: n x 48 B Zcash-flag compressed G1 keys; msg_pts: n x
- * 192 B messages ALREADY HASHED to G2, in the affine G2 packing (hash-to-curve is not part of the library).
+ * 192 B messages ALREADY HASHED to G2, in the affine G2 packing (nmsm_bls12_381_hash_to_g2_batch computes them;
+ * nmsm_bls12_381_verify_msg_batch takes the message bytes instead).
  * out_ok[i] = 1 iff pk decodes, is not the identity and is in G1, sig decodes, is not the identity and is in G2, H is
  * not the identity, and e(pk, H) e(-G1, sig) == 1.  Everything about a signature's or key's content is a 0 verdict,
  * never an error.  H comes from the caller's hash-to-curve and is in G2 by construction, so it is only checked for
@@ -308,6 +311,30 @@ int nmsm_bn254_pairing_check_batch(const uint8_t* g1_xy, const uint8_t* g2_xy, c
  * k_bls_verify_prepare in slot 0, k_bls_miller in slot 1, k_bls_final in slot 2 and their sum in NMSM_T_TOTAL. */
 int nmsm_bls12_381_verify_batch(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msg_pts, uint64_t n,
                                 uint8_t* out_ok);
+
+/* BLS12-381 hash to G2 (next-row f10): out_xy[i] = hash_to_curve(msg_i) on BLS12-381 G2, suite
+ * BLS12381G2_XMD:SHA-256_SSWU_RO_ (RFC 9380 §8.8.2; noble's bls12_381.G2.hashToCurve(msg, { DST })): expand_message_xmd
+ * with SHA-256, hash_to_field to two Fp2 elements, the simplified SWU map on the 3-isogenous curve and the isogeny, the
+ * sum of the two points, and cofactor clearing by h_eff.  message i = msgs[msg_off[i], msg_off[i+1]), any length
+ * including 0; dst: the domain separation tag, dst_len >= 1 bytes (noble's default for long signatures is
+ * "BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_NUL_", Ethereum's "..._POP_"); a tag over 255 bytes is replaced by
+ * SHA-256("H2C-OVERSIZE-DST-" || DST) (RFC 9380 §5.3.3).  out_xy: n x 192 B in the affine G2 packing (x.c0, x.c1,
+ * y.c0, y.c1, 48 B little-endian each); the points are in G2; the identity, which only arises with negligible
+ * probability, is written as (0, 0).  NMSM_ERR_ARG for null pointers, an empty tag, offsets that do not start at 0 or
+ * decrease, and n >= 2^30.  n == 0 writes nothing.  With profiling on, nmsm_last_timing reports k_bls_hash_to_g2 in
+ * slot 0 and in NMSM_T_TOTAL. */
+int nmsm_bls12_381_hash_to_g2_batch(const uint8_t* msgs, const uint64_t* msg_off, uint64_t n, const uint8_t* dst,
+                                    uint64_t dst_len, uint8_t* out_xy);
+
+/* nmsm_bls12_381_verify_batch with message i = msgs[msg_off[i], msg_off[i+1]) hashed to G2 on the GPU under dst, as
+ * nmsm_bls12_381_hash_to_g2_batch hashes it: out_ok[i] = bls12_381.verify(sig_i, G2.hashToCurve(msg_i, { DST }), pk_i).
+ * Every verdict rule of nmsm_bls12_381_verify_batch holds; the message points are in G2 by construction, so there is
+ * no message-point error.  NMSM_ERR_ARG as for nmsm_bls12_381_hash_to_g2_batch.  With profiling on, nmsm_last_timing
+ * reports k_bls_hash_to_g2 in slot 0, k_bls_verify_prepare in slot 1, k_bls_miller in slot 2, k_bls_final in slot 3
+ * and their sum in NMSM_T_TOTAL. */
+int nmsm_bls12_381_verify_msg_batch(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msgs,
+                                    const uint64_t* msg_off, uint64_t n, const uint8_t* dst, uint64_t dst_len,
+                                    uint8_t* out_ok);
 
 /* Batched wire-format decoding on the GPU (next-row f2): encodings -> canonical affine points in the packing
  * above, ready for nmsm_msm.  secp256k1: 33-byte SEC1 compressed (weierstrass.ts:565-588); BLS12-381 G1: 48-byte

@@ -167,6 +167,16 @@ inline int cuda_fail(cudaError_t e, const char* what) {
     if (e__ != cudaSuccess) return cuda_fail(e__, #call); \
   } while (0)
 
+// the offsets drive device reads of the concatenated keys / messages: they must start at 0 and never decrease
+inline int check_offsets(const uint64_t* off, const char* name, uint64_t n) {
+  if (off[0] != 0) return fail(NMSM_ERR_ARG, std::string(name) + "[0] must be 0");
+  for (uint64_t i = 0; i < n; i++)
+    if (off[i + 1] < off[i])
+      return fail(NMSM_ERR_ARG, std::string(name) + " must be non-decreasing (index " + std::to_string(i + 1) + ")",
+                  (long long)(i + 1));
+  return NMSM_OK;
+}
+
 inline int ensure_init() {
   if (g_ctx.ready) return NMSM_OK;
   return fail(NMSM_ERR_CUDA, "nmsm_init() has not been called (no CUDA context; there is no CPU fallback)");
@@ -217,6 +227,11 @@ int bn254_pairing_check_batch_impl(const uint8_t* g1_xy, const uint8_t* g2_xy, c
                                    uint64_t n_checks, uint8_t* out_ok);
 int bls12_381_verify_batch_impl(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msg_pts, uint64_t n,
                                 uint8_t* out_ok);
+int bls12_381_verify_msg_batch_impl(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msgs,
+                                    const uint64_t* msg_off, uint64_t n, const uint8_t* dst, uint64_t dst_len,
+                                    uint8_t* out_ok);
+int bls12_381_hash_to_g2_batch_impl(const uint8_t* msgs, const uint64_t* msg_off, uint64_t n, const uint8_t* dst,
+                                    uint64_t dst_len, uint8_t* out_xy);
 int decode_points_impl(int curve, const uint8_t* enc, uint64_t n, int flags, uint8_t* out_xy, uint8_t* out_status);
 int ntt_impl(int curve, void* values, int on_device, int log_n, uint64_t generator, int inverse, int brp_input,
              int brp_output);

@@ -1,9 +1,13 @@
-// BLS12-381 pairing checks and BLS signature verification (SURVEY §8 row f7, pairing.cuh): the kernels and the two
-// C-ABI implementations.  The chunked check driver is pairing_driver.cuh's (shared with bn254):
+// BLS12-381 pairing checks, BLS signature verification (SURVEY §8 row f7, pairing.cuh) and hash to G2 (f10,
+// hash_to_curve.cuh): the kernels and the four C-ABI implementations.  The chunked check driver is pairing_driver.cuh's
+// (shared with bn254):
+//   k_bls_hash_to_g2      (hash, verify_msg) one thread per message: RFC 9380 hash_to_curve, affine through one
+//                         inversion per warp
 //   k_bls_verify_prepare  (verify only) one thread per signature: decode, subgroup checks, the two pairs
 //   k_bls_miller          one thread per pair: validation and f_i = f_{|x|,Q_i}(P_i) into the workspace
 //   k_bls_final           one thread per check: the product of its f_i, the final exponentiation, the verdict
 // The Miller values of at most PAIRING_CHUNK pairs are alive at once (PAIRING_CHUNK x 576 B = 37.7 MB).
+#include "hash_to_curve.cuh"
 #include "pairing.cuh"
 #include "pairing_driver.cuh"
 
@@ -32,8 +36,106 @@ k_bls_verify_prepare(uint32_t n, const uint8_t* __restrict__ sigs, const uint8_t
   if (i < n) bls_verify_prepare_body(i, sigs, pks, msg_pts, g1, g2, pre_ok, err);
 }
 
+// Lanes past n feed the identity, whose inversion target is 1, to the warp-shared inversion.
+__global__ void __launch_bounds__(128)
+k_bls_hash_to_g2(uint32_t n, const uint8_t* __restrict__ msgs, const uint64_t* __restrict__ msg_off,
+                 const uint8_t* __restrict__ dst, uint32_t dlen, uint32_t* __restrict__ out) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  H2cG::Acc q = H2cG::identity();
+  if (i < n) q = h2c_hash_body(i, msgs, msg_off, dst, dlen);
+  const H2cF2 zi = warp_batch_inverse(H2cG::inv_target(q));
+  if (i < n) h2c_store(i, q, zi, out);
+}
+
 namespace {
 const PairingKernels BLS_KERNELS{k_bls_miller, k_bls_final};
+
+// messages hashed to G2 on the device: msgs / msg_off as the C ABI takes them, the tag already at most H2C_MAX_DST bytes
+struct BlsMessages {
+  const uint8_t* msgs;
+  const uint64_t* msg_off;
+  const uint8_t* dst;
+  uint32_t dlen;
+};
+
+// the tag of RFC 9380 §5.3.3: a DST over 255 bytes is replaced by SHA-256("H2C-OVERSIZE-DST-" || DST)
+BlsMessages bls_messages(const uint8_t* msgs, const uint64_t* msg_off, const uint8_t* dst, uint64_t dst_len,
+                         std::vector<uint8_t>& tag) {
+  if (dst_len <= H2C_MAX_DST) return BlsMessages{msgs, msg_off, dst, (uint32_t)dst_len};
+  static const char PREFIX[] = "H2C-OVERSIZE-DST-";
+  std::vector<uint8_t> in(PREFIX, PREFIX + sizeof(PREFIX) - 1);
+  in.insert(in.end(), dst, dst + dst_len);
+  tag.resize(32);
+  sha256(in.data(), in.size(), tag.data());
+  return BlsMessages{msgs, msg_off, tag.data(), 32};
+}
+
+// workspace bytes of bls_hash_launch for n messages
+uint64_t bls_hash_bytes(const BlsMessages& m, uint64_t n) { return al256(m.msg_off[n] + 16) + al256(8 * (n + 1)) + 256; }
+
+// uploads the messages, offsets and tag to ws (bls_hash_bytes) and runs k_bls_hash_to_g2 into d_out (timing slot 0)
+int bls_hash_launch(Context& X, Slot& C, const BlsMessages& m, uint64_t n, uint8_t* ws, uint32_t* d_out) {
+  cudaStream_t st = C.stream;
+  const uint64_t msg_bytes = m.msg_off[n], o_mo = al256(msg_bytes + 16), o_dst = o_mo + al256(8 * (n + 1));
+  if (msg_bytes)
+    if (int r = h2d_any(ws, m.msgs, msg_bytes, st)) return r;
+  if (int r = h2d_any(ws + o_mo, m.msg_off, 8 * (n + 1), st)) return r;
+  if (int r = h2d_any(ws + o_dst, m.dst, m.dlen, st)) return r;
+  return pairing_launch(X, C, 0, [&] {
+    k_bls_hash_to_g2<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, ws, (const uint64_t*)(ws + o_mo), ws + o_dst, m.dlen,
+                                                   d_out);
+  });
+}
+
+// nmsm_bls12_381_verify_batch (msg_pts on the host) and nmsm_bls12_381_verify_msg_batch (hm: the messages, hashed
+// into the same workspace by k_bls_hash_to_g2, which shifts the other kernels' timing slots by one)
+int bls_verify_impl(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msg_pts, const BlsMessages* hm,
+                    uint64_t n, uint8_t* out_ok) {
+  Context& X = g_ctx;
+  Slot& C = X.slot[0];
+  if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n must be < 2^30");
+  if (X.profiling) memset(X.last_ms, 0, sizeof(X.last_ms));
+  const uint64_t o_sig = 0, o_pk = o_sig + al256(96 * n), o_h = o_pk + al256(48 * n), o_g1 = o_h + al256(192 * n),
+                 o_g2 = o_g1 + al256(192 * n), o_pre = o_g2 + al256(384 * n),
+                 o_w = o_pre + al256(n), o_ok = o_w + al256(pairing_workspace_bytes<BlsPairing>()),
+                 o_misc = o_ok + al256(n), o_hash = o_misc + 256, bytes = o_hash + (hm ? bls_hash_bytes(*hm, n) : 0);
+  CK(X.ed_scratch.ensure(bytes));
+  uint8_t* base = (uint8_t*)X.ed_scratch.p;
+  cudaStream_t st = C.stream;
+  const int s0 = hm ? 1 : 0;
+  if (int r = h2d_any(base + o_sig, sigs96, 96 * n, st)) return r;
+  if (int r = h2d_any(base + o_pk, pks48, 48 * n, st)) return r;
+  if (hm) {
+    if (int r = bls_hash_launch(X, C, *hm, n, base + o_hash, (uint32_t*)(base + o_h))) return r;
+  } else if (int r = h2d_any(base + o_h, msg_pts, 192 * n, st)) {
+    return r;
+  }
+  unsigned int* d_err = (unsigned int*)(base + o_misc);
+  uint32_t *d_g1 = (uint32_t*)(base + o_g1), *d_g2 = (uint32_t*)(base + o_g2);
+  uint8_t *d_pre = base + o_pre, *d_ok = base + o_ok;
+  CK(cudaMemsetAsync(d_err, 0xff, 16, st));
+  if (int r = pairing_launch(X, C, s0, [&] {
+        k_bls_verify_prepare<<<cdiv(n, PAIRING_BLOCK), PAIRING_BLOCK, 0, st>>>(
+            (uint32_t)n, base + o_sig, base + o_pk, (const uint32_t*)(base + o_h), d_g1, d_g2, d_pre, d_err);
+      }))
+    return r;
+  if (int r = pairing_checks_run<BlsPairing>(X, C, BLS_KERNELS, n, nullptr, nullptr, d_g1, d_g2, d_pre,
+                                              (uint32_t*)(base + o_w), d_ok, d_err + 2, 1 + s0))
+    return r;
+  unsigned int err[4];
+  CK(cudaMemcpyAsync(err, d_err, 16, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (err[0] != 0xffffffffu)  // hashed messages are on the twist by construction
+    return fail(hm ? NMSM_ERR_CUDA : NMSM_ERR_POINT,
+                (hm ? "internal error: hashed message point " : "message point ") + std::to_string(err[0]) +
+                    " is out of range or not on the twist",
+                err[0]);
+  if (err[2] != 0xffffffffu || err[3] != 0xffffffffu)  // prepare only emits valid or identity pairs
+    return fail(NMSM_ERR_CUDA, "internal error: a prepared pair failed validation");
+  CK(cudaMemcpy(out_ok, d_ok, n, cudaMemcpyDeviceToHost));
+  return NMSM_OK;
+}
 }  // namespace
 
 int bls12_381_pairing_check_batch_impl(const uint8_t* g1_xy, const uint8_t* g2_xy, const uint64_t* pair_off,
@@ -43,42 +145,36 @@ int bls12_381_pairing_check_batch_impl(const uint8_t* g1_xy, const uint8_t* g2_x
 
 int bls12_381_verify_batch_impl(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msg_pts, uint64_t n,
                                 uint8_t* out_ok) {
+  return bls_verify_impl(sigs96, pks48, msg_pts, nullptr, n, out_ok);
+}
+
+int bls12_381_verify_msg_batch_impl(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msgs,
+                                    const uint64_t* msg_off, uint64_t n, const uint8_t* dst, uint64_t dst_len,
+                                    uint8_t* out_ok) {
+  if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n must be < 2^30");
+  if (int r = check_offsets(msg_off, "msg_off", n)) return r;
+  std::vector<uint8_t> tag;
+  const BlsMessages hm = bls_messages(msgs, msg_off, dst, dst_len, tag);
+  return bls_verify_impl(sigs96, pks48, nullptr, &hm, n, out_ok);
+}
+
+int bls12_381_hash_to_g2_batch_impl(const uint8_t* msgs, const uint64_t* msg_off, uint64_t n, const uint8_t* dst,
+                                    uint64_t dst_len, uint8_t* out_xy) {
   Context& X = g_ctx;
   Slot& C = X.slot[0];
   if (n == 0) return NMSM_OK;
   if (n >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n must be < 2^30");
+  if (int r = check_offsets(msg_off, "msg_off", n)) return r;
+  std::vector<uint8_t> tag;
+  const BlsMessages hm = bls_messages(msgs, msg_off, dst, dst_len, tag);
   if (X.profiling) memset(X.last_ms, 0, sizeof(X.last_ms));
-  const uint64_t o_sig = 0, o_pk = o_sig + al256(96 * n), o_h = o_pk + al256(48 * n), o_g1 = o_h + al256(192 * n),
-                 o_g2 = o_g1 + al256(192 * n), o_pre = o_g2 + al256(384 * n),
-                 o_w = o_pre + al256(n), o_ok = o_w + al256(pairing_workspace_bytes<BlsPairing>()),
-                 o_misc = o_ok + al256(n), bytes = o_misc + 256;
+  const uint64_t o_out = 0, o_hash = al256(192 * n), bytes = o_hash + bls_hash_bytes(hm, n);
   CK(X.ed_scratch.ensure(bytes));
   uint8_t* base = (uint8_t*)X.ed_scratch.p;
-  cudaStream_t st = C.stream;
-  if (int r = h2d_any(base + o_sig, sigs96, 96 * n, st)) return r;
-  if (int r = h2d_any(base + o_pk, pks48, 48 * n, st)) return r;
-  if (int r = h2d_any(base + o_h, msg_pts, 192 * n, st)) return r;
-  unsigned int* d_err = (unsigned int*)(base + o_misc);
-  uint32_t *d_g1 = (uint32_t*)(base + o_g1), *d_g2 = (uint32_t*)(base + o_g2);
-  uint8_t *d_pre = base + o_pre, *d_ok = base + o_ok;
-  CK(cudaMemsetAsync(d_err, 0xff, 16, st));
-  if (int r = pairing_launch(X, C, 0, [&] {
-        k_bls_verify_prepare<<<cdiv(n, PAIRING_BLOCK), PAIRING_BLOCK, 0, st>>>(
-            (uint32_t)n, base + o_sig, base + o_pk, (const uint32_t*)(base + o_h), d_g1, d_g2, d_pre, d_err);
-      }))
-    return r;
-  if (int r = pairing_checks_run<BlsPairing>(X, C, BLS_KERNELS, n, nullptr, nullptr, d_g1, d_g2, d_pre,
-                                              (uint32_t*)(base + o_w), d_ok, d_err + 2, 1))
-    return r;
-  unsigned int err[4];
-  CK(cudaMemcpyAsync(err, d_err, 16, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (err[0] != 0xffffffffu)
-    return fail(NMSM_ERR_POINT,
-                "message point " + std::to_string(err[0]) + " is out of range or not on the twist", err[0]);
-  if (err[2] != 0xffffffffu || err[3] != 0xffffffffu)  // prepare only emits valid or identity pairs
-    return fail(NMSM_ERR_CUDA, "internal error: a prepared pair failed validation");
-  CK(cudaMemcpy(out_ok, d_ok, n, cudaMemcpyDeviceToHost));
+  if (int r = bls_hash_launch(X, C, hm, n, base + o_hash, (uint32_t*)(base + o_out))) return r;
+  CK(cudaMemcpyAsync(out_xy, base + o_out, 192 * n, cudaMemcpyDeviceToHost, C.stream));
+  CK(cudaStreamSynchronize(C.stream));
   return NMSM_OK;
 }
 

@@ -87,16 +87,6 @@ k_recover_check(uint32_t n, const uint32_t* __restrict__ g_tbl, const uint32_t* 
   if (i < n) recover_finish<LAYOUT>(i, q_ok, acc, zi, out, ok);
 }
 
-// the offsets drive device reads of the concatenated keys / messages: they must start at 0 and never decrease
-static int check_offsets(const uint64_t* off, const char* name, uint64_t n) {
-  if (off[0] != 0) return fail(NMSM_ERR_ARG, std::string(name) + "[0] must be 0");
-  for (uint64_t i = 0; i < n; i++)
-    if (off[i + 1] < off[i])
-      return fail(NMSM_ERR_ARG, std::string(name) + " must be non-decreasing (index " + std::to_string(i + 1) + ")",
-                  (long long)(i + 1));
-  return NMSM_OK;
-}
-
 // The fixed-point table of G that ECDSA and Schnorr verification share: d * 2^(16 j) * G, the table table_mul_body
 // walks.  Built by the first verify after nmsm_init, freed by nmsm_shutdown.
 static int ensure_secp256k1_g_table(Context& X) {

@@ -1152,6 +1152,24 @@ def bls_verify_batch(signatures, message_points, public_keys) -> List[bool]:
     n = len(signatures)
     if len(message_points) != n or len(public_keys) != n:
         raise ValueError("signatures, messages and public keys must have equal length")
+    G2 = bls12_381.G2.Point
+    sigs, pks = _bls_sigs_and_keys(signatures, public_keys)
+    for m in message_points:
+        if isinstance(m, (bytes, bytearray, memoryview, str)):
+            raise NotImplementedError("hash-to-curve is not implemented: pass the message hashed to G2 as a "
+                                      "bls12_381.G2.Point")
+        if not isinstance(m, G2):
+            raise TypeError('"message" expected bls12_381.G2.Point, got type=%s' % type(m).__name__)
+    try:
+        out = bls_verify_batch_packed(sigs, pks, _pack_points(message_points), n)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return [b == 1 for b in out]
+
+
+def _bls_sigs_and_keys(signatures, public_keys):
+    """the packed signature and key arguments of the verify entry points: 96-byte and 48-byte Zcash-flag compressed
+    encodings, or Points (encoded first)"""
     G1, G2 = bls12_381.G1.Point, bls12_381.G2.Point
     sigs, pks = [], []
     for s in signatures:
@@ -1170,17 +1188,7 @@ def bls_verify_batch(signatures, message_points, public_keys) -> List[bool]:
         if len(k) != 48:
             raise ValueError('"publicKey" expected Uint8Array of length 48, got length=%d' % len(k))
         pks.append(bytes(k))
-    for m in message_points:
-        if isinstance(m, (bytes, bytearray, memoryview, str)):
-            raise NotImplementedError("hash-to-curve is not implemented: pass the message hashed to G2 as a "
-                                      "bls12_381.G2.Point")
-        if not isinstance(m, G2):
-            raise TypeError('"message" expected bls12_381.G2.Point, got type=%s' % type(m).__name__)
-    try:
-        out = bls_verify_batch_packed(b"".join(sigs), b"".join(pks), _pack_points(message_points), n)
-    except NmsmError as e:
-        _raise_mapped(e)
-    return [b == 1 for b in out]
+    return b"".join(sigs), b"".join(pks)
 
 
 def bls_verify_batch_packed(sigs96: bytes, pks48: bytes, msg_pts: bytes, n: int) -> bytes:
@@ -1202,6 +1210,105 @@ def _bls_verify(signature, message, publicKey) -> bool:
 
 
 bls12_381.verify = _bls_verify
+
+
+# ---- BLS12-381 hash to G2 (include/nmsm.h nmsm_bls12_381_hash_to_g2_batch, nmsm_bls12_381_verify_msg_batch) ------
+DST_G2_NUL = b"BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_NUL_"  # noble's default tag for long signatures
+DST_G2_POP = b"BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_POP_"  # proof-of-possession scheme (Ethereum consensus)
+
+
+def _h2c_args(messages, dst):
+    """(message bytes list, tag bytes) after the checks noble's hashToCurve makes: bytes messages, a non-empty tag
+    (a str tag is UTF-8, as noble accepts strings)"""
+    if isinstance(dst, str):
+        dst = dst.encode()
+    if not isinstance(dst, (bytes, bytearray, memoryview)):
+        raise TypeError('"DST" expected Uint8Array or string, got type=%s' % type(dst).__name__)
+    if len(dst) == 0:
+        raise ValueError("DST must be non-empty (RFC 9380 §3.1)")
+    msgs = []
+    for m in messages:
+        if not isinstance(m, (bytes, bytearray, memoryview)):
+            raise TypeError('"message" expected Uint8Array, got type=%s' % type(m).__name__)
+        msgs.append(bytes(m))
+    return msgs, bytes(dst)
+
+
+def bls_hash_to_g2_batch(messages, dst=DST_G2_NUL) -> List:
+    """Batch form of bls12_381.G2.hashToCurve(msg, { DST }) (RFC 9380 suite BLS12381G2_XMD:SHA-256_SSWU_RO_): one
+    bls12_381.G2.Point per message, each in G2.  Messages are bytes of any length; the tag is non-empty bytes (or str),
+    one tag for the whole batch."""
+    msgs, dst = _h2c_args(messages, dst)
+    if not msgs:
+        return []
+    xy = bls_hash_to_g2_batch_packed(b"".join(msgs), _pack_offsets(msgs), len(msgs), dst)
+    G2 = bls12_381.G2.Point
+    out = []
+    for k in range(len(msgs)):
+        b = xy[192 * k:192 * k + 192]
+        out.append(G2.from_packed(b, not any(b), valid=True))
+    return out
+
+
+def bls_hash_to_g2_batch_packed(msgs: bytes, msg_off: bytes, n: int, dst: bytes) -> bytes:
+    """The C-ABI call itself (nmsm_bls12_381_hash_to_g2_batch): the concatenated messages with n+1 little-endian u64
+    offsets and the tag.  Returns n*192 bytes of affine G2 points; raises NmsmError (with .code) on an error."""
+    if len(msg_off) != 8 * (n + 1):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(192 * n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    _lib.check(lib.nmsm_bls12_381_hash_to_g2_batch(cp(msgs or b"\0"), cp(msg_off), n, cp(dst or b"\0"), len(dst), out))
+    return out.raw[:192 * n]
+
+
+def _g2_hash_to_curve(msg, options=None):
+    """bls12_381.G2.hashToCurve(msg, { DST }) for one message (the batch entry point with n = 1); the default tag is
+    noble's BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_NUL_."""
+    dst = DST_G2_NUL
+    if options is not None:
+        if not isinstance(options, dict):
+            raise TypeError("options expected dict, got type=%s" % type(options).__name__)
+        dst = options.get("DST", DST_G2_NUL)
+    return bls_hash_to_g2_batch([msg], dst)[0]
+
+
+bls12_381.G2.hashToCurve = _g2_hash_to_curve
+
+
+def bls_verify_messages_batch(signatures, messages, public_keys, dst=DST_G2_NUL) -> List[bool]:
+    """bls_verify_batch with message bytes, hashed to G2 on the GPU under dst in the same call: verdict i is
+    bls12_381.verify(signature_i, G2.hashToCurve(message_i, { DST }), publicKey_i).  Signatures and keys as for
+    bls_verify_batch; a signature or key that does not decode, is the identity or lies outside its subgroup is a False
+    verdict."""
+    n = len(signatures)
+    if len(messages) != n or len(public_keys) != n:
+        raise ValueError("signatures, messages and public keys must have equal length")
+    msgs, dst = _h2c_args(messages, dst)
+    sigs, pks = _bls_sigs_and_keys(signatures, public_keys)
+    if n == 0:
+        return []
+    try:
+        out = bls_verify_messages_batch_packed(sigs, pks, b"".join(msgs), _pack_offsets(msgs), n, dst)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return [b == 1 for b in out]
+
+
+def bls_verify_messages_batch_packed(sigs96: bytes, pks48: bytes, msgs: bytes, msg_off: bytes, n: int,
+                                     dst: bytes) -> bytes:
+    """The C-ABI call itself (nmsm_bls12_381_verify_msg_batch): n*96 signature bytes, n*48 key bytes, the concatenated
+    messages with n+1 little-endian u64 offsets and the tag.  Returns n verdict bytes; raises NmsmError on an error."""
+    if len(sigs96) != 96 * n or len(pks48) != 48 * n or len(msg_off) != 8 * (n + 1):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    _lib.check(lib.nmsm_bls12_381_verify_msg_batch(cp(sigs96 or b"\0"), cp(pks48 or b"\0"), cp(msgs or b"\0"),
+                                                   cp(msg_off), n, cp(dst or b"\0"), len(dst), out))
+    return out.raw[:n]
 
 
 # ---- bn254 pairing checks (include/nmsm.h nmsm_bn254_pairing_check_batch) and EIP-197 ecPairing ---------------------
