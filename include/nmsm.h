@@ -199,7 +199,9 @@ int nmsm_point_table_mul_batch(uint64_t handle, const uint8_t* scalars, uint64_t
  * tables :230-312, loops :422-480).  `values`: 2^log_n elements of 32 bytes, canonical little-endian (< r),
  * transformed in place.  curve: NMSM_BN254_G1/G2 (Fr of bn254, 2-adicity 28) or NMSM_BLS12_381_G1/G2 (2-adicity 32).
  * generator: the non-residue G of rootsOfUnity (the reference's tests pass 7); 0 = findGenerator's choice
- * (fft.ts:175-180: 5 for both fields).  inverse = 0: direct(values, brp_input, brp_output), out[k] = a(omega^k);
+ * (fft.ts:175-180: 5 for both fields).  The argument is G mod r and must fit in 64 bits: a caller holding a larger G
+ * reduces it mod r first and cannot pass one whose residue is 0 or >= 2^64 (the Python mirror raises ValueError for
+ * those rather than truncate them).  inverse = 0: direct(values, brp_input, brp_output), out[k] = a(omega^k);
  * inverse = 1: inverse(values, brp_input, brp_output) incl. the 1/n scaling.  An element >= r is reported as
  * NMSM_ERR_SCALAR with its index and leaves `values` untouched. */
 int nmsm_ntt(int curve, uint8_t* values, int log_n, uint64_t generator, int inverse, int brp_input, int brp_output);

@@ -188,6 +188,9 @@ static int ntt_run(int field_key, int two_adicity, uint64_t default_gen, void* v
   const size_t bytes = (size_t)n * 32;
   cudaStream_t st = C.stream;
   CK(X.ntt_aux.ensure((16 + 8 * 32) * 4 + 16));
+  // growing the root buffer discards its contents: forget the cached key first, so that a call failing between here and
+  // the table's rebuild (an allocation below) cannot leave a stale key naming a garbage table
+  if (bytes > X.ntt_roots.cap) X.ntt_key_bits = -1;
   CK(X.ntt_roots.ensure(bytes));
   CK(X.ntt_work.ensure(bytes));
   CK(X.ntt_tmp.ensure(bytes));
@@ -217,12 +220,10 @@ static int ntt_run(int field_key, int two_adicity, uint64_t default_gen, void* v
   const bool dit = brp_input && !brp_output;
   // split the log_n stages into ceil(log_n / NTT_MAX_STAGES) passes of (nearly) equal depth
   const int npass = log_n ? (log_n + NTT_MAX_STAGES - 1) / NTT_MAX_STAGES : 0;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CK(cudaFuncSetAttribute(k_ntt_pass<P, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (1 << NTT_TILE_LOG) * 32));
-    CK(cudaFuncSetAttribute(k_ntt_pass<P, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (1 << NTT_TILE_LOG) * 32));
-    attr_set = true;
-  }
+  // the 64 KB opt-in is a property of the current device's context, not of the process: set it on every call (a few
+  // microseconds) so that a context re-bound to another device by nmsm_shutdown / nmsm_init has it too
+  CK(cudaFuncSetAttribute(k_ntt_pass<P, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (1 << NTT_TILE_LOG) * 32));
+  CK(cudaFuncSetAttribute(k_ntt_pass<P, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (1 << NTT_TILE_LOG) * 32));
   for (int k = 0; k < npass; k++) {
     // DIF consumes stages from the top, DIT from the bottom; pass k covers stages (lo, hi]
     const int a = (int)((long long)log_n * k / npass), b = (int)((long long)log_n * (k + 1) / npass);
