@@ -28,6 +28,7 @@
  *   nmsm_bls12_381_pairing_check_batch / nmsm_bn254_pairing_check_batch <- pairingBatch(...) == 1, one verdict per check
  *   nmsm_bls12_381_hash_to_g2_batch <- bls12_381.G2.hashToCurve(msg, { DST }) over a batch (RFC 9380)
  *   nmsm_bls12_381_verify_msg_batch <- bls12_381.verify over a batch with the messages hashed on the GPU
+ *   nmsm_bls12_381_aggregate_verify_batch <- FastAggregateVerify / bls.verifyBatch over a batch of checks
  *   nmsm_ntt           <- FFT(rootsOfUnity(Fr, G), Fr).direct / .inverse   src/abstract/fft.ts:518-575
  *
  * Data formats (all little-endian, plain bytes, caller-owned):
@@ -337,6 +338,32 @@ int nmsm_bls12_381_hash_to_g2_batch(const uint8_t* msgs, const uint64_t* msg_off
 int nmsm_bls12_381_verify_msg_batch(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msgs,
                                     const uint64_t* msg_off, uint64_t n, const uint8_t* dst, uint64_t dst_len,
                                     uint8_t* out_ok);
+
+/* BLS12-381 aggregate verification (next-row f3): FastAggregateVerify (one message, the keys of its N signers) and
+ * noble's bls.verifyBatch(signature, messages, publicKeys) (pairs sharing a message have their keys summed), over a
+ * batch of checks.
+ *   check j: signature sigs96[96 j ..] (Zcash-flag compressed G2) and groups [group_off[j], group_off[j+1]);
+ *   group g: message msgs[msg_off[g], msg_off[g+1]), hashed under dst exactly as nmsm_bls12_381_hash_to_g2_batch
+ *            hashes it (a tag over 255 bytes included), and keys [key_off[g], key_off[g+1]) of keys_xy;
+ *   key:     96 B affine G1 in the NMSM_BLS12_381_G1 packing (x || y, 48 B little-endian each), (0, 0) the identity.
+ * out_ok[j] = 1 iff (1) the signature decodes, is not the identity and lies in G2 (the rules of
+ * nmsm_bls12_381_verify_batch); (2) the check has at least one group and every group at least one key; (3) no key of the
+ * check is the identity; (4) no group's key sum S_g is the identity (IETF KeyValidate of the aggregate key); and
+ * (5) e(-G1, sig) prod_g e(S_g, H(m_g)) == 1.  Everything about content is a 0 verdict, never an error.
+ * Keys come DECODED AND SUBGROUP-CHECKED BY THE CALLER and are not subgroup-checked here (as with NMSM_BLS12_381_G1 and
+ * the pairing check): a consensus client validates each validator key once and caches it (nmsm_points_decode +
+ * nmsm_points_torsion_free do that on the GPU), and a per-call G1 subgroup check would cost about 300 times the key
+ * addition.  A key outside G1 gives whatever the formulas give.
+ * NMSM_ERR_POINT, with nmsm_last_error_index = the smallest global key index, for a key with a coordinate >= p or off
+ * the curve.  NMSM_ERR_ARG for null pointers where the data is non-empty, any of the three offset arrays not starting
+ * at 0 or decreasing, an empty tag, n_checks >= 2^30, n_groups + n_checks >= 2^31 (n_groups = group_off[n_checks]) and
+ * n_keys >= 2^31 (n_keys = key_off[n_groups]).  n_checks == 0 writes nothing.  With profiling on, nmsm_last_timing
+ * reports k_bls_hash_to_g2 in slot 0, both key-sum kernels in slot 1, k_bls_agg_prepare in slot 2, k_bls_miller in
+ * slot 3, k_bls_final in slot 4 and their sum in NMSM_T_TOTAL. */
+int nmsm_bls12_381_aggregate_verify_batch(const uint8_t* sigs96, const uint64_t* group_off, uint64_t n_checks,
+                                          const uint8_t* msgs, const uint64_t* msg_off, const uint8_t* keys_xy,
+                                          const uint64_t* key_off, const uint8_t* dst, uint64_t dst_len,
+                                          uint8_t* out_ok);
 
 /* Batched wire-format decoding on the GPU (next-row f2): encodings -> canonical affine points in the packing
  * above, ready for nmsm_msm.  secp256k1: 33-byte SEC1 compressed (weierstrass.ts:565-588); BLS12-381 G1: 48-byte

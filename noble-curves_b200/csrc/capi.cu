@@ -876,6 +876,22 @@ int nmsm_bls12_381_verify_msg_batch(const uint8_t* sigs96, const uint8_t* pks48,
   return bls12_381_verify_msg_batch_impl(sigs96, pks48, msgs, msg_off, n, dst, dst_len, out_ok);
 }
 
+int nmsm_bls12_381_aggregate_verify_batch(const uint8_t* sigs96, const uint64_t* group_off, uint64_t n_checks,
+                                          const uint8_t* msgs, const uint64_t* msg_off, const uint8_t* keys_xy,
+                                          const uint64_t* key_off, const uint8_t* dst, uint64_t dst_len,
+                                          uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (!dst) return fail(NMSM_ERR_ARG, "null pointer");
+  if (dst_len == 0) return fail(NMSM_ERR_ARG, "dst must not be empty");
+  if (n_checks == 0) return NMSM_OK;
+  if (!sigs96 || !group_off || !msg_off || !key_off || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
+  return bls12_381_aggregate_verify_batch_impl(sigs96, group_off, n_checks, msgs, msg_off, keys_xy, key_off, dst,
+                                               dst_len, out_ok);
+}
+
 int nmsm_points_decode_ex(int curve, const uint8_t* enc, uint64_t n, int flags, uint8_t* out_xy, uint8_t* out_status) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (int r = ensure_init()) return r;

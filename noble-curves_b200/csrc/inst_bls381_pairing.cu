@@ -1,12 +1,16 @@
-// BLS12-381 pairing checks, BLS signature verification (SURVEY §8 row f7, pairing.cuh) and hash to G2 (f10,
-// hash_to_curve.cuh): the kernels and the four C-ABI implementations.  The chunked check driver is pairing_driver.cuh's
-// (shared with bn254):
-//   k_bls_hash_to_g2      (hash, verify_msg) one thread per message: RFC 9380 hash_to_curve, affine through one
-//                         inversion per warp
+// BLS12-381 pairing checks, BLS signature verification (SURVEY §8 row f7, pairing.cuh), hash to G2 (f10,
+// hash_to_curve.cuh) and aggregate verification (f3, bls_aggregate.cuh): the kernels and the five C-ABI
+// implementations.  The chunked check driver is pairing_driver.cuh's (shared with bn254):
+//   k_bls_hash_to_g2      (hash, verify_msg, aggregate) one thread per message: RFC 9380 hash_to_curve, affine through
+//                         one inversion per warp
 //   k_bls_verify_prepare  (verify only) one thread per signature: decode, subgroup checks, the two pairs
+//   k_bls_key_tiles       (aggregate only) one warp per tile of keys of one group: the partial key sums
+//   k_bls_key_groups      (aggregate only) one thread per group: its key sum S_g and the pair (S_g, H(m_g))
+//   k_bls_agg_prepare     (aggregate only) one thread per check: signature decode and subgroup check, the pair (-G1, sig)
 //   k_bls_miller          one thread per pair: validation and f_i = f_{|x|,Q_i}(P_i) into the workspace
 //   k_bls_final           one thread per check: the product of its f_i, the final exponentiation, the verdict
 // The Miller values of at most PAIRING_CHUNK pairs are alive at once (PAIRING_CHUNK x 576 B = 37.7 MB).
+#include "bls_aggregate.cuh"
 #include "hash_to_curve.cuh"
 #include "pairing.cuh"
 #include "pairing_driver.cuh"
@@ -47,8 +51,55 @@ k_bls_hash_to_g2(uint32_t n, const uint8_t* __restrict__ msgs, const uint64_t* _
   if (i < n) h2c_store(i, q, zi, out);
 }
 
+// one warp per tile (4 per block): lane sums, then a shuffle tree whose lane 0 writes the partial and the bad flag
+__global__ void __launch_bounds__(128)
+k_bls_key_tiles(uint32_t n_tiles, const BlsKeyTile* __restrict__ tiles, const uint32_t* __restrict__ keys,
+                uint32_t* __restrict__ partials, uint8_t* __restrict__ tile_bad, unsigned int* err) {
+  const uint32_t t = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (t >= n_tiles) return;  // the whole warp
+  bool bad = false;
+  BlsG1::Acc acc = bls_key_lane(tiles[t], lane, keys, bad, err);
+  for (uint32_t d = BLS_KEY_LANES / 2; d; d >>= 1) {
+    const int src = lane + d < 32 ? lane + d : lane;
+    const BlsG1::Acc o{shfl_field(acc.X, src), shfl_field(acc.Y, src), shfl_field(acc.ZZ, src), shfl_field(acc.ZZZ, src)};
+    BlsG1::add(acc, o);
+  }
+  bad = __any_sync(0xffffffffu, bad);
+  if (lane == 0) {
+    uint32_t w[BLS_ACC_WORDS];
+    BlsG1::store_acc(w, acc);
+    store_words<BLS_ACC_WORDS>(partials + (size_t)t * BLS_ACC_WORDS, w);
+    tile_bad[t] = bad ? 1 : 0;
+  }
+}
+
+// one thread per group; lanes past n and bad groups feed 1 to the warp-shared inversion
+__global__ void __launch_bounds__(128)
+k_bls_key_groups(uint32_t n_groups, const uint32_t* __restrict__ tile_off, const uint32_t* __restrict__ partials,
+                 const uint8_t* __restrict__ tile_bad, const uint32_t* __restrict__ group_pair,
+                 const uint32_t* __restrict__ h, uint32_t* __restrict__ g1, uint32_t* __restrict__ g2,
+                 uint8_t* __restrict__ group_ok) {
+  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  bool ok = false;
+  BlsG1::Acc s = BlsG1::identity();
+  if (g < n_groups) s = bls_group_sum(g, tile_off, partials, tile_bad, ok);
+  const BlsF zi = warp_batch_inverse(ok ? s.ZZZ : BlsF::one());
+  if (g < n_groups) bls_group_store(g, group_pair[g], ok, s, zi, h, g1, g2, group_ok);
+}
+
+__global__ void __launch_bounds__(PAIRING_BLOCK)
+k_bls_agg_prepare(uint32_t n, const uint8_t* __restrict__ sigs, const uint64_t* __restrict__ group_off,
+                  const uint8_t* __restrict__ group_ok, uint32_t* __restrict__ g1, uint32_t* __restrict__ g2,
+                  uint8_t* __restrict__ pre_ok) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < n) bls_agg_prepare_body(j, sigs, group_off, group_ok, g1, g2, pre_ok);
+}
+
 namespace {
 const PairingKernels BLS_KERNELS{k_bls_miller, k_bls_final};
+
+// keys per tile of k_bls_key_tiles, and the most tiles one group is split into (bls_key_tiles)
+constexpr uint64_t BLS_KEY_TILE = 128, BLS_KEY_TILE_CAP = 256;
 
 // messages hashed to G2 on the device: msgs / msg_off as the C ABI takes them, the tag already at most H2C_MAX_DST bytes
 struct BlsMessages {
@@ -136,7 +187,102 @@ int bls_verify_impl(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* 
   CK(cudaMemcpy(out_ok, d_ok, n, cudaMemcpyDeviceToHost));
   return NMSM_OK;
 }
+
+// nmsm_bls12_381_aggregate_verify_batch after the argument checks of capi.cu: 0 < n < 2^30, the offsets checked,
+// n_groups + n < 2^31 and n_keys < 2^31
+int bls_aggregate_impl(const uint8_t* sigs96, const uint64_t* group_off, uint64_t n, const BlsMessages& hm,
+                       const uint8_t* keys_xy, const uint64_t* key_off, uint8_t* out_ok) {
+  Context& X = g_ctx;
+  Slot& C = X.slot[0];
+  const uint64_t n_groups = group_off[n], n_keys = n_groups ? key_off[n_groups] : 0, n_pairs = n_groups + n;
+  if (n_groups == 0) {  // every check is empty
+    memset(out_ok, 0, n);
+    return NMSM_OK;
+  }
+  if (X.profiling) memset(X.last_ms, 0, sizeof(X.last_ms));
+  std::vector<BlsKeyTile> tiles;
+  std::vector<uint32_t> tile_off, group_pair(n_groups);
+  bls_key_tiles(key_off, n_groups, BLS_KEY_TILE, BLS_KEY_TILE_CAP, tiles, tile_off);
+  std::vector<uint64_t> pair_off(n + 1);
+  for (uint64_t j = 0; j <= n; j++) pair_off[j] = group_off[j] + j;
+  for (uint64_t j = 0; j < n; j++)
+    for (uint64_t g = group_off[j]; g < group_off[j + 1]; g++) group_pair[g] = (uint32_t)(g + j);
+  const uint64_t nt = tiles.size();
+  const uint64_t o_sig = 0, o_goff = o_sig + al256(96 * n), o_poff = o_goff + al256(8 * (n + 1)),
+                 o_keys = o_poff + al256(8 * (n + 1)), o_tiles = o_keys + al256(96 * n_keys),
+                 o_toff = o_tiles + al256(8 * nt), o_gpair = o_toff + al256(4 * (n_groups + 1)),
+                 o_part = o_gpair + al256(4 * n_groups), o_tbad = o_part + al256(4 * BLS_ACC_WORDS * nt),
+                 o_h = o_tbad + al256(nt), o_g1 = o_h + al256(192 * n_groups), o_g2 = o_g1 + al256(96 * n_pairs),
+                 o_gok = o_g2 + al256(192 * n_pairs), o_pre = o_gok + al256(n_groups), o_w = o_pre + al256(n),
+                 o_ok = o_w + al256(pairing_workspace_bytes<BlsPairing>()), o_misc = o_ok + al256(n),
+                 o_hash = o_misc + 256, bytes = o_hash + bls_hash_bytes(hm, n_groups);
+  CK(X.ed_scratch.ensure(bytes));
+  uint8_t* base = (uint8_t*)X.ed_scratch.p;
+  cudaStream_t st = C.stream;
+  if (int r = h2d_any(base + o_sig, sigs96, 96 * n, st)) return r;
+  if (int r = h2d_any(base + o_goff, group_off, 8 * (n + 1), st)) return r;
+  if (int r = h2d_any(base + o_poff, pair_off.data(), 8 * (n + 1), st)) return r;
+  if (n_keys)
+    if (int r = h2d_any(base + o_keys, keys_xy, 96 * n_keys, st)) return r;
+  if (nt)
+    if (int r = h2d_any(base + o_tiles, tiles.data(), 8 * nt, st)) return r;
+  if (int r = h2d_any(base + o_toff, tile_off.data(), 4 * (n_groups + 1), st)) return r;
+  if (int r = h2d_any(base + o_gpair, group_pair.data(), 4 * n_groups, st)) return r;
+  unsigned int* d_err = (unsigned int*)(base + o_misc);
+  CK(cudaMemsetAsync(d_err, 0xff, 16, st));
+  uint32_t *d_h = (uint32_t*)(base + o_h), *d_g1 = (uint32_t*)(base + o_g1), *d_g2 = (uint32_t*)(base + o_g2),
+           *d_part = (uint32_t*)(base + o_part);
+  uint8_t *d_tbad = base + o_tbad, *d_gok = base + o_gok, *d_pre = base + o_pre, *d_ok = base + o_ok;
+  if (int r = bls_hash_launch(X, C, hm, n_groups, base + o_hash, d_h)) return r;
+  if (nt)
+    if (int r = pairing_launch(X, C, 1, [&] {
+          k_bls_key_tiles<<<cdiv(nt, 4), 128, 0, st>>>((uint32_t)nt, (const BlsKeyTile*)(base + o_tiles),
+                                                       (const uint32_t*)(base + o_keys), d_part, d_tbad, d_err);
+        }))
+      return r;
+  if (int r = pairing_launch(X, C, 1, [&] {
+        k_bls_key_groups<<<cdiv(n_groups, 128), 128, 0, st>>>((uint32_t)n_groups, (const uint32_t*)(base + o_toff),
+                                                              d_part, d_tbad, (const uint32_t*)(base + o_gpair), d_h,
+                                                              d_g1, d_g2, d_gok);
+      }))
+    return r;
+  if (int r = pairing_launch(X, C, 2, [&] {
+        k_bls_agg_prepare<<<cdiv(n, PAIRING_BLOCK), PAIRING_BLOCK, 0, st>>>(
+            (uint32_t)n, base + o_sig, (const uint64_t*)(base + o_goff), d_gok, d_g1, d_g2, d_pre);
+      }))
+    return r;
+  if (int r = pairing_checks_run<BlsPairing>(X, C, BLS_KERNELS, n, pair_off.data(), (const uint64_t*)(base + o_poff),
+                                              d_g1, d_g2, d_pre, (uint32_t*)(base + o_w), d_ok, d_err + 2, 3))
+    return r;
+  unsigned int err[4];
+  CK(cudaMemcpyAsync(err, d_err, 16, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (err[0] != 0xffffffffu)
+    return fail(NMSM_ERR_POINT, "key " + std::to_string(err[0]) + " is out of range or not on the curve", err[0]);
+  if (err[2] != 0xffffffffu || err[3] != 0xffffffffu)  // key sums and hashed messages are on their curves
+    return fail(NMSM_ERR_CUDA, "internal error: an aggregate pair failed validation");
+  CK(cudaMemcpy(out_ok, d_ok, n, cudaMemcpyDeviceToHost));
+  return NMSM_OK;
+}
 }  // namespace
+
+int bls12_381_aggregate_verify_batch_impl(const uint8_t* sigs96, const uint64_t* group_off, uint64_t n_checks,
+                                          const uint8_t* msgs, const uint64_t* msg_off, const uint8_t* keys_xy,
+                                          const uint64_t* key_off, const uint8_t* dst, uint64_t dst_len,
+                                          uint8_t* out_ok) {
+  if (n_checks == 0) return NMSM_OK;
+  if (n_checks >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n_checks must be < 2^30");
+  if (int r = check_offsets(group_off, "group_off", n_checks)) return r;
+  const uint64_t n_groups = group_off[n_checks];
+  if (n_groups >= (1ull << 31) - n_checks) return fail(NMSM_ERR_ARG, "the number of pairs must be < 2^31");
+  if (int r = check_offsets(msg_off, "msg_off", n_groups)) return r;
+  if (int r = check_offsets(key_off, "key_off", n_groups)) return r;
+  if (key_off[n_groups] >= (1ull << 31)) return fail(NMSM_ERR_ARG, "the number of keys must be < 2^31");
+  if ((msg_off[n_groups] && !msgs) || (key_off[n_groups] && !keys_xy)) return fail(NMSM_ERR_ARG, "null pointer");
+  std::vector<uint8_t> tag;
+  const BlsMessages hm = bls_messages(msgs, msg_off, dst, dst_len, tag);
+  return bls_aggregate_impl(sigs96, group_off, n_checks, hm, keys_xy, key_off, out_ok);
+}
 
 int bls12_381_pairing_check_batch_impl(const uint8_t* g1_xy, const uint8_t* g2_xy, const uint64_t* pair_off,
                                        uint64_t n_checks, uint8_t* out_ok) {

@@ -1311,6 +1311,149 @@ def bls_verify_messages_batch_packed(sigs96: bytes, pks48: bytes, msgs: bytes, m
     return out.raw[:n]
 
 
+# ---- BLS12-381 aggregate verification (include/nmsm.h nmsm_bls12_381_aggregate_verify_batch) ------------------------
+def _bls_agg_layout(checks):
+    """checks[j] = (signature, [(message bytes, [public keys]), ...]) -> (signature bytes, group offsets, messages, key
+    offsets, keys as given).  Type and length checks only; no device."""
+    G2 = bls12_381.G2.Point
+    sigs, group_off, msgs, key_off, keys = [], [0], [], [0], []
+    for j, check in enumerate(checks):
+        if not isinstance(check, (tuple, list)) or len(check) != 2:
+            raise TypeError("check %d: (signature, [(message, [public keys]), ...]) expected" % j)
+        s, groups = check
+        sigs.append(s)
+        for group in groups:
+            if not isinstance(group, (tuple, list)) or len(group) != 2:
+                raise TypeError("check %d: (message, [public keys]) groups expected" % j)
+            m, ks = group
+            if isinstance(m, G2):
+                raise TypeError("check %d: messages are hashed here: pass the message bytes, not a G2 Point" % j)
+            msgs.append(m)
+            keys.extend(ks)
+            key_off.append(len(keys))
+        group_off.append(len(msgs))
+    return sigs, group_off, msgs, key_off, keys
+
+
+def _bls_agg_keys(keys) -> bytes:
+    """the 96-byte affine packing of public keys (48-byte encodings or G1 Points), every one decoded and subgroup-checked
+    on the GPU unless it is a Point known valid; a key that fails is packed as the identity, which fails its check"""
+    G1 = bls12_381.G1.Point
+    for k in keys:
+        if isinstance(k, G1):
+            continue
+        if not isinstance(k, (bytes, bytearray, memoryview)):
+            raise TypeError('"publicKey" expected Uint8Array or G1 Point, got type=%s' % type(k).__name__)
+        if len(k) != 48:
+            raise ValueError('"publicKey" expected Uint8Array of length 48, got length=%d' % len(k))
+    ident = bytes(96)
+    packed = {}  # unique encodings and Points to check -> packed key
+    encs = sorted({bytes(k) for k in keys if not isinstance(k, G1)})
+    if encs:
+        xy, st = points_decode(BLS12_381_G1, b"".join(encs), len(encs))
+        ok = torsion_free_packed(BLS12_381_G1, xy, len(encs))
+        for i, e in enumerate(encs):
+            packed[e] = xy[96 * i:96 * i + 96] if st[i] == 1 and ok[i] == 1 else ident
+    pts = [k for k in keys if isinstance(k, G1) and not k._valid and not k.is0()]
+    if pts:
+        raw = _pack_points(pts)
+        on = points_on_curve(BLS12_381_G1, raw, len(pts))
+        ok = torsion_free_packed(BLS12_381_G1, raw, len(pts))
+        for i, p in enumerate(pts):
+            packed[id(p)] = raw[96 * i:96 * i + 96] if on[i] == 1 and ok[i] == 1 else ident
+    out = []
+    for k in keys:
+        if not isinstance(k, G1):
+            out.append(packed[bytes(k)])
+        elif k.is0():
+            out.append(ident)
+        else:
+            out.append(packed.get(id(k)) or k.to_packed())
+    return b"".join(out)
+
+
+def bls_aggregate_verify_batch(checks, dst=DST_G2_NUL) -> List[bool]:
+    """Aggregate verification over a batch: checks[j] = (signature, [(message bytes, [public keys]), ...]), verdict j is
+    e(-G1, sig) prod_g e(sum of group g's keys, hashToCurve(m_g, { DST })) == 1 (noble's verifyBatch with the keys of
+    each message summed; one group is FastAggregateVerify).  Signatures are 96-byte encodings or G2 Points, keys 48-byte
+    encodings or G1 Points.  A signature or key that does not decode, is the identity or lies outside its subgroup, an
+    empty check or group, and a group whose keys sum to the identity are a False verdict.  Byte keys are decoded and
+    subgroup-checked once per distinct encoding on the GPU; Points not known valid are checked likewise."""
+    checks = list(checks)
+    sigs, group_off, msgs, key_off, keys = _bls_agg_layout(checks)
+    msgs, dst = _h2c_args(msgs, dst)
+    sigs96, _ = _bls_sigs_and_keys(sigs, [])
+    if not checks:
+        return []
+    import struct
+
+    pack = lambda v: struct.pack("<%dQ" % len(v), *v)  # noqa: E731
+    try:
+        out = bls_aggregate_verify_batch_packed(sigs96, pack(group_off), b"".join(msgs), _pack_offsets(msgs),
+                                                _bls_agg_keys(keys), pack(key_off), len(checks), dst)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return [b == 1 for b in out]
+
+
+def bls_aggregate_verify_batch_packed(sigs96: bytes, group_off: bytes, msgs: bytes, msg_off: bytes, keys_xy: bytes,
+                                      key_off: bytes, n_checks: int, dst: bytes) -> bytes:
+    """The C-ABI call itself (nmsm_bls12_381_aggregate_verify_batch): n_checks*96 signature bytes, n_checks+1 group
+    offsets, the concatenated messages with n_groups+1 offsets, 96-byte affine keys with n_groups+1 key offsets (all
+    offsets little-endian u64) and the tag.  Returns n_checks verdict bytes; raises NmsmError on an error."""
+    if len(sigs96) != 96 * n_checks or len(group_off) != 8 * (n_checks + 1):
+        raise ValueError("packed arrays do not match n_checks")
+    n_groups = int.from_bytes(group_off[-8:], "little")
+    if len(msg_off) != 8 * (n_groups + 1) or len(key_off) != 8 * (n_groups + 1):
+        raise ValueError("packed arrays do not match the group count")
+    if len(keys_xy) != 96 * int.from_bytes(key_off[-8:], "little"):
+        raise ValueError("packed arrays do not match the key count")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n_checks, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    _lib.check(lib.nmsm_bls12_381_aggregate_verify_batch(cp(sigs96 or b"\0"), cp(group_off), n_checks,
+                                                         cp(msgs or b"\0"), cp(msg_off), cp(keys_xy or b"\0"),
+                                                         cp(key_off), cp(dst or b"\0"), len(dst), out))
+    return out.raw[:n_checks]
+
+
+def bls_fast_aggregate_verify_batch(signatures, messages, public_keys, dst=DST_G2_POP) -> List[bool]:
+    """Ethereum's FastAggregateVerify over a batch: verdict j checks signatures[j] over messages[j] against the sum of
+    public_keys[j] (a list of keys), under the proof-of-possession tag by default.  Rules as bls_aggregate_verify_batch;
+    an empty key list is False."""
+    n = len(signatures)
+    if len(messages) != n or len(public_keys) != n:
+        raise ValueError("signatures, messages and public keys must have equal length")
+    return bls_aggregate_verify_batch([(s, [(m, list(ks))]) for s, m, ks in zip(signatures, messages, public_keys)],
+                                      dst)
+
+
+def _bls_verify_batch_groups(messages, publicKeys):
+    """noble's verifyBatch pairing of keys with messages: one group per distinct message, in first-seen order"""
+    if len(messages) != len(publicKeys):
+        raise ValueError("messages and publicKeys must have equal length")
+    groups = {}
+    for m, k in zip(messages, publicKeys):
+        if isinstance(m, bls12_381.G2.Point):
+            raise TypeError("verifyBatch hashes the messages: pass the message bytes, not a G2 Point")
+        if not isinstance(m, (bytes, bytearray, memoryview)):
+            raise TypeError('"message" expected Uint8Array, got type=%s' % type(m).__name__)
+        groups.setdefault(bytes(m), []).append(k)
+    return list(groups.items())
+
+
+def _bls_verify_batch(signature, messages, publicKeys) -> bool:
+    """bls12_381.verifyBatch(signature, messages, publicKeys) (abstract/bls.ts): one aggregate signature over (message,
+    key) pairs, messages as bytes hashed under DST_G2_NUL.  Pairs with equal message bytes form one group whose keys are
+    summed.  noble groups by message object identity instead; the verdicts differ in one place: a key and its negation
+    under the same message bytes sum to the identity here, which is False (IETF KeyValidate of the aggregate key)."""
+    return bls_aggregate_verify_batch([(signature, _bls_verify_batch_groups(messages, publicKeys))])[0]
+
+
+bls12_381.verifyBatch = _bls_verify_batch
+
+
 # ---- bn254 pairing checks (include/nmsm.h nmsm_bn254_pairing_check_batch) and EIP-197 ecPairing ---------------------
 def bn254_pairing_check_batch(checks) -> List[bool]:
     """pairing_check_batch on bn254: checks[j] is a list of (bn254.G1.Point, bn254.G2.Point) pairs, True iff the

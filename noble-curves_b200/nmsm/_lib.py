@@ -43,7 +43,7 @@ EXPORTS = [
     "nmsm_secp256k1_verify_batch", "nmsm_secp256k1_schnorr_verify_batch",
     "nmsm_secp256k1_recover_batch", "nmsm_secp256k1_ecrecover_batch",
     "nmsm_bls12_381_pairing_check_batch", "nmsm_bls12_381_verify_batch", "nmsm_bn254_pairing_check_batch",
-    "nmsm_bls12_381_hash_to_g2_batch", "nmsm_bls12_381_verify_msg_batch",
+    "nmsm_bls12_381_hash_to_g2_batch", "nmsm_bls12_381_verify_msg_batch", "nmsm_bls12_381_aggregate_verify_batch",
 ]
 
 
@@ -186,6 +186,9 @@ def load() -> ctypes.CDLL:
         lib.nmsm_bls12_381_hash_to_g2_batch.restype = ctypes.c_int
         lib.nmsm_bls12_381_verify_msg_batch.argtypes = [u8p, u8p, u8p, u8p, ctypes.c_uint64, u8p, ctypes.c_uint64, u8p]
         lib.nmsm_bls12_381_verify_msg_batch.restype = ctypes.c_int
+        lib.nmsm_bls12_381_aggregate_verify_batch.argtypes = [u8p, u8p, ctypes.c_uint64, u8p, u8p, u8p, u8p, u8p,
+                                                              ctypes.c_uint64, u8p]
+        lib.nmsm_bls12_381_aggregate_verify_batch.restype = ctypes.c_int
         lib.nmsm_msm_submit.argtypes = [ctypes.c_int, u8p, u8p, ctypes.c_uint64, ctypes.c_int, ctypes.c_int]
         lib.nmsm_msm_submit.restype = ctypes.c_int
         lib.nmsm_msm_collect.argtypes = [ctypes.c_int, u8p, ctypes.POINTER(ctypes.c_int)]
