@@ -144,15 +144,25 @@ struct SwXyzz {
     p.X = X3;
     p.Y = Y3;
   }
-  // p += a (affine): madd-2008-s with the exceptional cases handled explicitly
+  // p += a (affine): madd-2008-s with the exceptional cases handled explicitly.  INL: the field products of the
+  // general case are expanded in place (field.cuh mul_inline), for k_accumulate's loop; the rare doubling stays shared.
+  template <bool INL = false>
   NMSM_HD static void madd(Acc& p, const Affine& a) {
+    auto mul = [](const F& x, const F& y) -> F {
+      if constexpr (INL) return mul_inline(x, y);
+      else return x * y;
+    };
+    auto sq = [](const F& x) -> F {
+      if constexpr (INL) return sqr_inline(x);
+      else return sqr(x);
+    };
     if (affine_is_identity(a)) return;
     if (is_identity(p)) {
       p = Acc{a.x, a.y, F::one(), F::one()};
       return;
     }
-    F U2 = a.x * p.ZZ;
-    F S2 = a.y * p.ZZZ;
+    F U2 = mul(a.x, p.ZZ);
+    F S2 = mul(a.y, p.ZZZ);
     F P = U2 - p.X;
     F R = S2 - p.Y;
     if (P.is_zero()) {
@@ -162,13 +172,13 @@ struct SwXyzz {
         p = identity();
       return;
     }
-    F PP = sqr(P);
-    F PPP = P * PP;
-    F Q = p.X * PP;
-    F X3 = sqr(R) - PPP - nmsm::dbl(Q);
-    F Y3 = R * (Q - X3) - p.Y * PPP;
-    p.ZZ = p.ZZ * PP;
-    p.ZZZ = p.ZZZ * PPP;
+    F PP = sq(P);
+    F PPP = mul(P, PP);
+    F Q = mul(p.X, PP);
+    F X3 = sq(R) - PPP - nmsm::dbl(Q);
+    F Y3 = mul(R, Q - X3) - mul(p.Y, PPP);
+    p.ZZ = mul(p.ZZ, PP);
+    p.ZZZ = mul(p.ZZZ, PPP);
     p.X = X3;
     p.Y = Y3;
   }

@@ -393,6 +393,21 @@ NMSM_HD Fp<C> sqr(const Fp<C>& a) {
   return r;
 #endif
 }
+// a * b and a^2 with the Montgomery body expanded at the call site whatever NMSM_MUL_NOINLINE says.  For the hot loop of
+// k_accumulate only: a call to the shared out-of-line body passes its operands and result through a fixed register ABI,
+// and what is live across the call spills (for 381-bit XYZZ, on every product of every mixed addition).
+template <class C>
+NMSM_HD Fp<C> mul_inline(const Fp<C>& a, const Fp<C>& b) {
+  Fp<C> r;
+  mont_mul<C>(r.v, a.v, b.v);
+  return r;
+}
+template <class C>
+NMSM_HD Fp<C> sqr_inline(const Fp<C>& a) {
+  Fp<C> r;
+  mont_sqr<C>(r.v, a.v);
+  return r;
+}
 template <class C>
 NMSM_HD Fp<C> dbl(const Fp<C>& a) {
   return a + a;

@@ -161,17 +161,8 @@ __device__ __noinline__ F warp_batch_inverse(const F& z) {
 #ifndef NMSM_PAIRED
 #define NMSM_PAIRED 0
 #endif
-#ifndef NMSM_ACC_MINBLOCKS_WIDE
-#define NMSM_ACC_MINBLOCKS_WIDE 2  // BLS12-381 G2: a 4-coordinate Fp2 accumulator alone is 96 registers
-#endif
-#ifndef NMSM_ACC_WIDE_BYTES
-#define NMSM_ACC_WIDE_BYTES 257  // accumulators from this size on take the WIDE occupancy
-#endif
-#ifndef NMSM_ACC_MINBLOCKS
-#define NMSM_ACC_MINBLOCKS 4  // 4 x 128 threads per SM: <= 128 registers per thread of the 64 K-register file
-#endif
 template <class Cv>
-__global__ void __launch_bounds__(128, (sizeof(typename Cv::G::Acc) >= NMSM_ACC_WIDE_BYTES ? NMSM_ACC_MINBLOCKS_WIDE : NMSM_ACC_MINBLOCKS))
+__global__ void __launch_bounds__(128, acc_blocks_per_sm<typename Cv::G>())
 k_accumulate(const uint32_t* __restrict__ aff, const uint32_t* __restrict__ sorted,
              const uint32_t* __restrict__ offsets, MsmPlan plan, uint32_t w0, uint32_t* __restrict__ buckets,
              uint32_t* __restrict__ heads, uint32_t* __restrict__ tails) {

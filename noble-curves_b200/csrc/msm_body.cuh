@@ -45,11 +45,28 @@ struct MsmPlan {
                     // (w, t) owns the sorted entries [offsets[w*B] + t*L, + L) of window w, so no segment straddles
                     // two windows and the windows can be accumulated and reduced as independent launches
 };
-// Entries per accumulate thread: whole waves of the grid (4 blocks of 128 threads per SM) with at most 64 entries per
-// thread.  Longer segments mean fewer bucket partials for k_reduce1 to stitch, and sizing them to fill the last wave
-// keeps k_accumulate's tail short.
-NMSM_HD int plan_seg_len(double entries, int sm_count) {
-  const double wave = (double)sm_count * 4.0 * 128.0;  // threads of one full wave
+// Blocks of 128 threads per SM that k_accumulate is built for: its __launch_bounds__ (so 65536 / (128 * blocks)
+// registers per thread) and the wave that plan_seg_len sizes the segments for.  By accumulator size:
+//   128 B  XYZZ over a 256-bit field, ed25519 extended coordinates   4 blocks, <= 128 registers
+//   192 B  XYZZ over the 381-bit BLS12-381 field                      3 blocks, <= 168 registers: the mixed addition
+//          with inline products (ec.cuh madd<true>) fits without local memory; under 128 registers it spills
+//   256 B  bn254 G2 (XYZZ over Fp2, 254 bits)                         4 blocks
+//   384 B  BLS12-381 G2 (XYZZ over Fp2, 381 bits)                     2 blocks: the accumulator alone is 96 registers
+template <class G>
+NMSM_HD constexpr int acc_blocks_per_sm() {
+  return sizeof(typename G::Acc) == 192 ? 3 : (sizeof(typename G::Acc) > 256 ? 2 : 4);
+}
+// Inline products in k_accumulate's mixed addition where that budget holds them without spills.  Under 128 registers
+// (the 256-bit curves) the inline form spills more than the calls to the shared out-of-line body do.
+template <class G>
+NMSM_HD constexpr bool acc_inline_products() {
+  return acc_blocks_per_sm<G>() == 3;
+}
+// Entries per accumulate thread: whole waves of the grid (acc_blocks_per_sm blocks of 128 threads per SM) with at most
+// 64 entries per thread.  Longer segments mean fewer bucket partials for k_reduce1 to stitch, and sizing them to fill
+// the last wave keeps k_accumulate's tail short.
+NMSM_HD int plan_seg_len(double entries, int sm_count, int blocks_per_sm) {
+  const double wave = (double)sm_count * blocks_per_sm * 128.0;  // threads of one full wave
   const double waves = ceil(entries / (64.0 * wave));
   int L = (int)ceil(entries / ((waves < 1.0 ? 1.0 : waves) * wave));
   return L < 4 ? 4 : (L > 64 ? 64 : L);
@@ -99,7 +116,7 @@ inline MsmPlan make_plan(uint64_t n, int forced_c, int sm_count, uint64_t n_loca
   const double t_add_lat = 0.030 * fscale * G::COST_ADD / 14.0;          // ms, dependent chain (2 warps / sub-partition)
   const double t_dbl_par = 0.0062 * fscale;                              // ms per Horner doubling (lane-parallel)
   const int K = 8;
-  auto seg_len = [&](double entries) { return plan_seg_len(entries, sm_count); };
+  auto seg_len = [&](double entries) { return plan_seg_len(entries, sm_count, acc_blocks_per_sm<G>()); };
   int best_c = min_c;
   double best = 1e300;
   for (int c = min_c; c <= MAX_WINDOW_BITS; c++) {  // min_c: sharded MSMs run one launch group per window, keep W small
@@ -159,7 +176,7 @@ NMSM_HD bool reduce1_quad_form(const MsmPlan& p) { return p.stride == 0 && (uint
 template <class Cv>
 inline void plan_one_wave_per_window(MsmPlan& p, uint64_t n_local, int sm_count) {
   const double terms_local = (double)(n_local ? n_local : 1) * split_of<Cv>();
-  int L1 = (int)ceil(terms_local / ((double)sm_count * 4.0 * 128.0));
+  int L1 = (int)ceil(terms_local / ((double)sm_count * acc_blocks_per_sm<typename Cv::G>() * 128.0));
   p.L = L1 < 4 ? 4 : (L1 > 64 ? 64 : L1);
   p.TPW = plan_tpw((uint64_t)terms_local, p.L);
 }
@@ -208,7 +225,7 @@ inline int choose_table_bits(uint64_t n_points, int sm_count, double mem_budget_
     const int wb = T / D, r = T % D;
     const double B = (double)(1u << (c - 1));
     const double entries = terms * D;
-    const int L = plan_seg_len(entries, sm_count);
+    const int L = plan_seg_len(entries, sm_count, acc_blocks_per_sm<G>());
     // r digits are c bits wide, D - r only c - 1: the lower half of the buckets receives all D digits
     const double load_low = r ? terms * ((double)(D - r) / (double)(1u << (wb - 1)) + (double)r / (double)(1u << wb))
                               : entries / B;
@@ -240,7 +257,7 @@ inline MsmPlan make_table_plan(uint64_t n_points, int c, int sm_count) {
   p.B = 1 << (p.c - 1);
   p.G = p.B;
   p.stride = (uint32_t)(n_points * split_of<Cv>());
-  p.L = plan_seg_len(terms * p.D, sm_count);
+  p.L = plan_seg_len(terms * p.D, sm_count, acc_blocks_per_sm<typename Cv::G>());
   int Kc = TABLE_REDUCE_CHUNK;
 #if !defined(__CUDA_ARCH__)
   if (const char* e = getenv("NMSM_TK")) { int v = atoi(e); if (v >= 1 && (v & (v - 1)) == 0) Kc = v; }  // tuning experiments
@@ -299,6 +316,20 @@ NMSM_HD void load_words_rw(uint32_t* dst, const uint32_t* src) {
   for (int k = 0; k < WORDS; k++) dst[k] = src[k];
 #endif
 }
+#if defined(__CUDA_ARCH__)
+// Asynchronous copy of WORDS words (16-byte pieces) from global memory to dst[piece][threadIdx.x] in shared memory, as
+// one cp.async group: consecutive threads write consecutive 16 bytes, so the stores are free of bank conflicts.
+template <int WORDS>
+__device__ __forceinline__ void load_words_async(uint4 (*dst)[128], const uint32_t* src) {
+  static_assert(WORDS % 4 == 0, "rows are 16-byte multiples");
+#pragma unroll
+  for (int k = 0; k < WORDS / 4; k++) {
+    const uint32_t d = (uint32_t)__cvta_generic_to_shared(&dst[k][threadIdx.x]);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(src + 4 * k) : "memory");
+  }
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
+#endif
 template <int WORDS>
 NMSM_HD void store_words(uint32_t* dst, const uint32_t* src) {
 #if defined(__CUDA_ARCH__)
@@ -863,20 +894,57 @@ NMSM_HD void accumulate_body(uint32_t w, uint32_t t, const uint32_t* aff, const 
   uint32_t g = lo;
   uint32_t bstart = offsets[g], bend = offsets[g + 1];
   typename G::Acc acc = G::identity();
-  for (uint32_t pos = seg; pos < end; pos++) {
-    if (pos == bend) {
-      // bucket g is finished inside this segment
-      if (bstart >= seg) save_acc<G>(buckets + (size_t)g * G::ACC_WORDS, acc);
-      else save_acc<G>(heads + sid * G::ACC_WORDS, acc);
-      acc = G::identity();
-      do { g++; } while (offsets[g + 1] <= pos);
-      bstart = offsets[g];
-      bend = offsets[g + 1];
+  // bucket g is finished inside this segment at entry pos: flush it, move on to the bucket of pos
+  auto next_bucket = [&](uint32_t pos) {
+    if (bstart >= seg) save_acc<G>(buckets + (size_t)g * G::ACC_WORDS, acc);
+    else save_acc<G>(heads + sid * G::ACC_WORDS, acc);
+    acc = G::identity();
+    do { g++; } while (offsets[g + 1] <= pos);
+    bstart = offsets[g];
+    bend = offsets[g + 1];
+  };
+#if defined(__CUDA_ARCH__)
+  if constexpr (acc_inline_products<G>()) {
+    // The point of entry pos + 1 is requested before the addition of entry pos (cp.async into a per-thread double buffer
+    // in shared memory, 2 x AFF_WORDS words per thread, no registers), and the sorted index two entries ahead: the
+    // gathers' latency hides behind one mixed addition.  At 3 blocks per SM too few warps are resident to hide it.
+    // k_accumulate runs 128-thread blocks.
+    constexpr int Q = G::AFF_WORDS / 4;
+    __shared__ uint4 next_pts[2][Q][128];
+    uint32_t e = sorted[seg], e_next = seg + 1 < end ? sorted[seg + 1] : 0u;
+    load_words_async<G::AFF_WORDS>(next_pts[0], aff + (size_t)(e & 0x7fffffffu) * G::AFF_WORDS);
+    for (uint32_t pos = seg, slot = 0; pos < end; pos++, slot ^= 1u) {
+      if (pos == bend) next_bucket(pos);
+      const uint32_t e_after = pos + 2 < end ? sorted[pos + 2] : 0u;
+      if (pos + 1 < end) load_words_async<G::AFF_WORDS>(next_pts[slot ^ 1u], aff + (size_t)(e_next & 0x7fffffffu) * G::AFF_WORDS);
+      else asm volatile("cp.async.commit_group;" ::: "memory");  // empty group: the wait below then means "entry pos"
+      asm volatile("cp.async.wait_group 1;" ::: "memory");          // all groups but the newest are complete
+      typename G::Affine a;
+      uint32_t* aw = reinterpret_cast<uint32_t*>(&a);
+#pragma unroll
+      for (int k = 0; k < Q; k++) {
+        const uint4 v = next_pts[slot][k][threadIdx.x];
+        aw[4 * k] = v.x;
+        aw[4 * k + 1] = v.y;
+        aw[4 * k + 2] = v.z;
+        aw[4 * k + 3] = v.w;
+      }
+      a = G::cneg(a, (e >> 31) != 0);
+      G::template madd<true>(acc, a);
+      e = e_next;
+      e_next = e_after;
     }
-    uint32_t e = sorted[pos];
-    typename G::Affine a = load_aff<G>(aff + (size_t)(e & 0x7fffffffu) * G::AFF_WORDS);
-    a = G::cneg(a, (e >> 31) != 0);
-    G::madd(acc, a);
+  } else
+#endif
+  {
+    for (uint32_t pos = seg; pos < end; pos++) {
+      if (pos == bend) next_bucket(pos);
+      uint32_t e = sorted[pos];
+      typename G::Affine a = load_aff<G>(aff + (size_t)(e & 0x7fffffffu) * G::AFF_WORDS);
+      a = G::cneg(a, (e >> 31) != 0);
+      if constexpr (acc_inline_products<G>()) G::template madd<true>(acc, a);
+      else G::madd(acc, a);
+    }
   }
   const bool head_open = bstart < seg;
   const bool tail_open = bend > end;
