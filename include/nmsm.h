@@ -21,6 +21,7 @@
  *   nmsm_points_decode / nmsm_points_torsion_free  <- Point.fromBytes: decode + isTorsionFree
  *                                                                 weierstrass.ts:541-605,971-975, bls12-381.ts:377-468
  *   nmsm_ed25519_verify_batch <- ed25519.verify over a batch      edwards.ts:942-989
+ *   nmsm_ed25519_verify_each <- ed25519.verify over a batch, one verdict per signature (ZIP-215 or strict)
  *   nmsm_secp256k1_verify_batch <- secp256k1.verify over a batch, one verdict per signature (weierstrass.ts ecdsa().verify)
  *   nmsm_secp256k1_schnorr_verify_batch <- schnorr.verify over a batch, one verdict per signature (secp256k1.ts, BIP340)
  *   nmsm_secp256k1_recover_batch <- secp256k1.recoverPublicKey over a batch (weierstrass.ts Signature.recoverPublicKey)
@@ -219,6 +220,23 @@ int nmsm_ntt_device(int curve, void* d_values, int log_n, uint64_t generator, in
 int nmsm_ed25519_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint8_t* msgs,
                               const uint64_t* msg_off, uint64_t n, const uint8_t* z16, int* out_ok,
                               long long* out_bad_index);
+
+/* Ed25519 verification with one verdict per signature: out_ok[i] = ed25519.verify(sig_i, msg_i, pk_i, { zip215 })
+ * (edwards.ts:942-989).  nmsm_ed25519_verify_batch gives ONE verdict for the whole batch: a signature that decodes but
+ * is wrong (bad s, wrong message or key) fails the batch without saying which; this entry point says which.
+ * Per signature: A = decode(pk_i), R = decode(sig_i[0:32]); s = LE(sig_i[32:64]) < l (s = 0 allowed); under
+ * NMSM_ED25519_VERIFY_STRICT also [8]A != O; k = LE(SHA-512(sig_i[0:32] || pk_i || msg_i)) mod l over the bytes as
+ * given; accept iff [8](R + k A - s B) == O (cofactored in both modes).  flags 0 = { zip215: true }, noble's default
+ * for ed25519: any 255-bit y is reduced and x = 0 with the sign bit set is accepted.
+ * sigs: n x 64 B; pubkeys: n x 32 B; message i = msgs[msg_off[i], msg_off[i+1]), any length; out_ok: n bytes, 1 = valid.
+ * Everything about a signature's content (an undecodable R or A, s >= l, a small-order A in strict mode, a failed
+ * equation) is a 0 verdict, never an error; NMSM_ERR_ARG is for null pointers, offsets that do not start at 0 or
+ * decrease, unknown flag bits and n >= 2^31.  n == 0 writes nothing.  The first call after nmsm_init builds the
+ * fixed-point table of B (16 x 2^15 points, 48 MiB), kept until nmsm_shutdown.  With profiling on, nmsm_last_timing
+ * reports k_ed_verify_prepare in slot 0, k_ed_verify_check in slot 1 and both in NMSM_T_TOTAL. */
+#define NMSM_ED25519_VERIFY_STRICT 1 /* { zip215: false }: RFC 8032 decoding + small-order A rejected */
+int nmsm_ed25519_verify_each(const uint8_t* sigs, const uint8_t* pubkeys, const uint8_t* msgs, const uint64_t* msg_off,
+                             uint64_t n, int flags, uint8_t* out_ok);
 
 /* secp256k1 ECDSA batch verification (next-row f5): out_ok[i] = secp256k1.verify(sig_i, msg_i, pk_i, { prehash, lowS })
  * with format 'compact' (noble-curves weierstrass.ts ecdsa().verify), one independent verdict per signature.

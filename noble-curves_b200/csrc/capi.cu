@@ -421,6 +421,8 @@ void nmsm_shutdown(void) {
   C.ed_scratch.release();
   cudaFree(C.secp256k1_g_table);
   C.secp256k1_g_table = nullptr;
+  cudaFree(C.ed25519_b_table);
+  C.ed25519_b_table = nullptr;
   for (Buf* b : {&C.ntt_data, &C.ntt_work, &C.ntt_tmp, &C.ntt_roots, &C.ntt_aux}) b->release();
   C.ntt_key_field = -1;
   C.ntt_key_bits = -1;
@@ -758,6 +760,20 @@ int nmsm_ed25519_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const
     return fail(NMSM_ERR_ARG, "null pointer");
   if (n && msg_off[n] && !msgs) return fail(NMSM_ERR_ARG, "null pointer");
   return ed25519_verify_batch_impl(sigs, pubkeys, msgs, msg_off, n, z16, out_ok, out_bad_index);
+}
+
+int nmsm_ed25519_verify_each(const uint8_t* sigs, const uint8_t* pubkeys, const uint8_t* msgs, const uint64_t* msg_off,
+                             uint64_t n, int flags, uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (flags & ~NMSM_ED25519_VERIFY_STRICT) return fail(NMSM_ERR_ARG, "nmsm_ed25519_verify_each: unknown flag");
+  if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 31)) return fail(NMSM_ERR_ARG, "n must be < 2^31");  // before msg_off[n] is read
+  if (!sigs || !pubkeys || !msg_off || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
+  if (msg_off[n] && !msgs) return fail(NMSM_ERR_ARG, "null pointer");
+  return ed25519_verify_each_impl(sigs, pubkeys, msgs, msg_off, n, flags, out_ok);
 }
 
 int nmsm_secp256k1_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint64_t* pk_off, const uint8_t* msgs,

@@ -100,6 +100,7 @@ struct Context {
   int cur = 0;  // slot used by the call in progress (set by the C-ABI wrapper under the mutex)
   Buf ed_scratch;              // signature-verification scratch (ed25519 and secp256k1 batches)
   uint32_t* secp256k1_g_table = nullptr;  // fixed-point table of the secp256k1 generator, built by the first verify
+  uint32_t* ed25519_b_table = nullptr;    // fixed-point table of the ed25519 base point, built by the first verify_each
   Buf ntt_data, ntt_work, ntt_tmp, ntt_roots, ntt_aux;  // NTT staging / work / output / root table (ntt.cu)
   int ntt_key_field = -1, ntt_key_bits = -1;            // which root table ntt_roots holds
   uint64_t ntt_key_gen = 0;
@@ -177,6 +178,17 @@ inline int check_offsets(const uint64_t* off, const char* name, uint64_t n) {
   return NMSM_OK;
 }
 
+// with profiling on: the two kernels of a per-signature verify (events 0-1-2 of the slot) in timing slots 0, 1 and
+// NMSM_T_TOTAL
+inline void record_verify_timing(Context& X, Slot& C) {
+  if (!X.profiling) return;
+  memset(X.last_ms, 0, sizeof(X.last_ms));
+  cudaEventElapsedTime(&X.last_ms[0], C.ev[0], C.ev[1]);
+  cudaEventElapsedTime(&X.last_ms[1], C.ev[1], C.ev[2]);
+  cudaEventElapsedTime(&X.last_ms[NMSM_T_TOTAL], C.ev[0], C.ev[2]);
+  (void)cudaGetLastError();
+}
+
 inline int ensure_init() {
   if (g_ctx.ready) return NMSM_OK;
   return fail(NMSM_ERR_CUDA, "nmsm_init() has not been called (no CUDA context; there is no CPU fallback)");
@@ -214,6 +226,8 @@ struct EngineVTable {
 };
 int ed25519_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs, const uint64_t* msg_off,
                               uint64_t n, const uint8_t* z16, int* out_ok, long long* out_bad_index);
+int ed25519_verify_each_impl(const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs, const uint64_t* msg_off,
+                             uint64_t n, int flags, uint8_t* out_ok);
 int secp256k1_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off, const uint8_t* msgs,
                                 const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
 int secp256k1_schnorr_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs,

@@ -191,6 +191,19 @@ NMSM_HD EdS eds_to_mont(const uint32_t* x) {
   return a * r2;
 }
 
+// k = SHA-512(R || A || M) mod l in Montgomery form, over the signature's R bytes and the key bytes as given (not
+// re-encoded: ZIP-215 accepts non-canonical encodings, and the hash must see them as sent)
+NMSM_HD EdS ed_challenge(const uint8_t* r32, const uint8_t* a32, const uint8_t* msg, uint64_t mlen) {
+  uint8_t digest[64];
+  sha512_rAM(r32, a32, msg, mlen, digest);
+  uint32_t lo[8], hi[8];
+  words_from_le_bytes(lo, digest, 8);  // k = little-endian integer of the 64-byte digest (edwards.ts:867)
+  words_from_le_bytes(hi, digest + 32, 8);
+  EdS r2;
+  for (int k = 0; k < 8; k++) r2.v[k] = FnEd25519Mod::R2(k);
+  return eds_to_mont(lo) + eds_to_mont(hi) * r2;  // (lo + hi * 2^256) mod l
+}
+
 // Per-signature scalars.  Layout of the MSM that follows (2n+1 terms):
 //   points  [0,n) = R_i   [n,2n) = A_i   [2n] = B
 //   scalars [0,n) = z_i   [n,2n) = z_i*k_i mod l   [2n] = -(sum z_i*s_i) mod l
@@ -216,16 +229,10 @@ NMSM_HD void ed_terms_body(uint32_t i, uint32_t n, const uint8_t* sigs, const ui
     for (int k = 0; k < 8; k++) scalars[(size_t)i * 8 + k] = scalars[(size_t)(n + i) * 8 + k] = 0;
     return;
   }
-  uint8_t digest[64];
-  sha512_rAM(sig, pk, msgs + msg_off[i], msg_off[i + 1] - msg_off[i], digest);
-  uint32_t lo[8], hi[8], z[8];
-  words_from_le_bytes(lo, digest, 8);  // k = little-endian integer of the 64-byte digest (edwards.ts:867)
-  words_from_le_bytes(hi, digest + 32, 8);
+  const EdS k_m = ed_challenge(sig, pk, msgs + msg_off[i], msg_off[i + 1] - msg_off[i]);
+  uint32_t z[8];
   words_from_le_bytes(z, z16 + (size_t)i * 16, 4);
   for (int k = 4; k < 8; k++) z[k] = 0;
-  EdS r2;
-  for (int k = 0; k < 8; k++) r2.v[k] = FnEd25519Mod::R2(k);
-  const EdS k_m = eds_to_mont(lo) + eds_to_mont(hi) * r2;  // (lo + hi * 2^256) mod l, Montgomery form
   const EdS z_m = eds_to_mont(z);
   const EdS zk = z_m * k_m;
   const EdS zs = z_m * eds_to_mont(s);
@@ -254,6 +261,80 @@ NMSM_HD void ed_finish_serial(uint32_t n, const uint32_t* zs_mont, uint32_t* pts
     pts[(size_t)(2 * n) * 16 + k] = Ed25519Consts::GX(k);
     pts[(size_t)(2 * n) * 16 + 8 + k] = Ed25519Consts::GY(k);
   }
+}
+
+// ---- one verdict per signature (nmsm_ed25519_verify_each) ------------------------------------------------------
+// The batch equation above answers for the whole batch; a caller holding signatures from untrusted senders needs to
+// know WHICH one fails.  Per signature, as edwards.ts:942-989 states it:
+//   ed_verify_prepare_body  decode A and R, s < l, (strict) [8]A != O, k = SHA-512(R || A || M) mod l
+//   ed_verify_check_body    [8](s B - k A - R) == O: s B from the fixed-point table of B, k A by 4-bit signed windows
+// Two kernels (inst_ed25519.cu), as for ECDSA: the SHA-512 and square-root state stays out of the scalar
+// multiplication's registers.  No inversion: the identity test works on projective coordinates.
+static constexpr int ED_VERIFY_STRICT = 1;  // include/nmsm.h NMSM_ED25519_VERIFY_STRICT
+
+// [8]P == O for canonical affine (x, y): the strict mode's small-order test of A (verify's `!zip215 && A.isSmallOrder()`)
+NMSM_HD bool ed_small_order(const uint32_t* xy) {
+  using G = CurveEd25519::G;
+  G::Acc p = G::from_affine(G::prepare(xy));
+  for (int j = 0; j < 3; j++) nl_dbl<G>(p);
+  return G::is_identity(p);
+}
+
+// Signature i: A, R (canonical affine words), s and k (canonical words mod l), and the prepare verdict in ok_out[i].
+// flags & ED_VERIFY_STRICT: RFC 8032 decoding and small-order A rejected ({ zip215: false }); else ZIP-215 decoding.
+NMSM_HD void ed_verify_prepare_body(uint32_t i, const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs,
+                                    const uint64_t* msg_off, int flags, uint32_t* as, uint32_t* rs, uint32_t* ss,
+                                    uint32_t* ks, uint8_t* ok_out) {
+  const uint8_t* sig = sigs + (size_t)i * 64;
+  const uint8_t* pk = pks + (size_t)i * 32;
+  const bool zip215 = (flags & ED_VERIFY_STRICT) == 0;
+  uint32_t a[16], r[16], s[8];
+  bool ok = ed_decompress(pk, a, zip215);
+  ok = ed_decompress(sig, r, zip215) && ok;
+  words_from_le_bytes(s, sig + 32, 8);
+  ok = ok && EdS::canonical_in_range(s);  // s >= l is false; s = 0 is allowed (multiplyUnsafe, edwards.ts:573)
+  if (ok && !zip215 && ed_small_order(a)) ok = false;
+  ok_out[i] = ok ? 1 : 0;
+  if (!ok) return;
+  uint32_t k[8];
+  ed_challenge(sig, pk, msgs + msg_off[i], msg_off[i + 1] - msg_off[i]).to_canonical(k);
+  store_words<16>(as + (size_t)i * 16, a);
+  store_words<16>(rs + (size_t)i * 16, r);
+  store_words<8>(ss + (size_t)i * 8, s);
+  store_words<8>(ks + (size_t)i * 8, k);
+}
+
+// Signature i after the prepare: out_ok[i] = [8](s B - k A - R) == O, the cofactored equation of both modes.
+// tbl: the fixed-point table of B (table_mul_body layout, BITS-bit digits; BITS is a parameter only so that
+// tests/hostemu can use a small table).
+template <int BITS = PT_BITS>
+NMSM_HD void ed_verify_check_body(uint32_t i, const uint32_t* tbl, const uint32_t* as, const uint32_t* rs,
+                                  const uint32_t* ss, const uint32_t* ks, uint8_t* out_ok, unsigned int* err) {
+  using Cv = CurveEd25519;
+  using G = Cv::G;
+  if (!out_ok[i]) return;
+  G::Acc acc;
+  table_mul_body<Cv, BITS>(i, tbl, ss, 1, acc, err);  // s < l always; s = 0 gives O
+  uint32_t a[16], r[16], k[8];
+  load_words<16>(a, as + (size_t)i * 16);
+  load_words<16>(r, rs + (size_t)i * 16);
+  load_words<8>(k, ks + (size_t)i * 8);
+  nl_add<G>(acc, scalar_mul_acc<Cv>(G::neg(G::prepare(a)), k));  // complete formulas: any A, including small order
+  nl_madd<G>(acc, G::neg(G::prepare(r)));
+  for (int j = 0; j < 3; j++) nl_dbl<G>(acc);
+  out_ok[i] = G::is_identity(acc) ? 1 : 0;
+}
+
+// serial statements of k_ed_verify_prepare / k_ed_verify_check
+NMSM_HD void ed_verify_prepare_serial(uint32_t n, const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs,
+                                      const uint64_t* msg_off, int flags, uint32_t* as, uint32_t* rs, uint32_t* ss,
+                                      uint32_t* ks, uint8_t* ok_out) {
+  for (uint32_t i = 0; i < n; i++) ed_verify_prepare_body(i, sigs, pks, msgs, msg_off, flags, as, rs, ss, ks, ok_out);
+}
+template <int BITS = PT_BITS>
+NMSM_HD void ed_verify_check_serial(uint32_t n, const uint32_t* tbl, const uint32_t* as, const uint32_t* rs,
+                                    const uint32_t* ss, const uint32_t* ks, uint8_t* out_ok, unsigned int* err) {
+  for (uint32_t i = 0; i < n; i++) ed_verify_check_body<BITS>(i, tbl, as, rs, ss, ks, out_ok, err);
 }
 
 }  // namespace nmsm

@@ -98,16 +98,6 @@ static int ensure_secp256k1_g_table(Context& X) {
   return Engine<CurveSecp256k1>::build_point_table((const uint8_t*)g_xy, &X.secp256k1_g_table, &levels);
 }
 
-// with profiling on: the two kernels of a verify (events 0-1-2 of slot 0) in timing slots 0, 1 and NMSM_T_TOTAL
-static void record_verify_timing(Context& X, Slot& C) {
-  if (!X.profiling) return;
-  memset(X.last_ms, 0, sizeof(X.last_ms));
-  cudaEventElapsedTime(&X.last_ms[0], C.ev[0], C.ev[1]);
-  cudaEventElapsedTime(&X.last_ms[1], C.ev[1], C.ev[2]);
-  cudaEventElapsedTime(&X.last_ms[NMSM_T_TOTAL], C.ev[0], C.ev[2]);
-  (void)cudaGetLastError();
-}
-
 int secp256k1_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off, const uint8_t* msgs,
                                 const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok) {
   Context& X = g_ctx;

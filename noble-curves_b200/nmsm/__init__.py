@@ -873,6 +873,59 @@ def ed25519_verify_batch_packed(sigs: bytes, pks: bytes, msgs: bytes, msg_off: b
     return bool(ok.value), int(bad.value)
 
 
+ED25519_VERIFY_STRICT = 1  # include/nmsm.h NMSM_ED25519_VERIFY_STRICT
+
+
+def ed25519_verify_each(signatures, messages, public_keys, zip215: bool = True) -> List[bool]:
+    """ed25519.verify(sig, msg, publicKey, { zip215 }) (edwards.ts:942-989) for every signature of a batch: one verdict
+    per signature, unlike ed25519_verify_batch's single batch equation.  zip215 = True is noble's default for ed25519;
+    False is RFC 8032 decoding with small-order keys rejected.  Raises where the reference throws before its `try`
+    (non-bytes arguments, a signature that is not 64 bytes, a key that is not 32 bytes) and for lists of different
+    lengths; everything else (an undecodable R or key, s >= l, a small-order key in strict mode, a failed equation) is
+    a False verdict."""
+    n = len(signatures)
+    if len(messages) != n or len(public_keys) != n:
+        raise ValueError("signatures, messages and public keys must have equal length")
+    for what, items in (("signature", signatures), ("message", messages), ("publicKey", public_keys)):
+        for x in items:
+            if not isinstance(x, (bytes, bytearray, memoryview)):
+                raise TypeError('"%s" expected Uint8Array, got type=%s' % (what, type(x).__name__))
+    for what, items, size in (("signature", signatures, 64), ("publicKey", public_keys, 32)):
+        for x in items:
+            if len(x) != size:
+                raise ValueError('"%s" expected Uint8Array of length %d, got length=%d' % (what, size, len(x)))
+    out = ed25519_verify_each_packed(b"".join(bytes(s) for s in signatures), b"".join(bytes(p) for p in public_keys),
+                                     b"".join(bytes(m) for m in messages), _pack_offsets(messages), n, zip215)
+    return [b == 1 for b in out]
+
+
+def ed25519_verify_each_packed(sigs: bytes, pks: bytes, msgs: bytes, msg_off: bytes, n: int,
+                               zip215: bool = True) -> bytes:
+    """The C-ABI call itself (nmsm_ed25519_verify_each) on caller-packed arrays: n*64 signature bytes, n*32 key bytes,
+    the concatenated messages with n+1 little-endian u64 offsets.  Returns n verdict bytes (1 = valid)."""
+    if len(sigs) != 64 * n or len(pks) != 32 * n or len(msg_off) != 8 * (n + 1):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    rc = lib.nmsm_ed25519_verify_each(cp(sigs or b"\0"), cp(pks or b"\0"), cp(msgs or b"\0"), cp(msg_off), n,
+                                      0 if zip215 else ED25519_VERIFY_STRICT, out)
+    try:
+        _lib.check(rc)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return out.raw[:n]
+
+
+def _ed25519_verify(signature, message, publicKey, zip215: bool = True) -> bool:
+    """ed25519.verify for one signature (the per-signature entry point with n = 1)."""
+    return ed25519_verify_each([signature], [message], [publicKey], zip215=zip215)[0]
+
+
+ed25519.verify = _ed25519_verify
+
+
 ECDSA_PREHASH = 1  # include/nmsm.h NMSM_ECDSA_PREHASH
 ECDSA_LOW_S = 2  # include/nmsm.h NMSM_ECDSA_LOW_S
 

@@ -37,7 +37,7 @@ EXPORTS = [
     "nmsm_mul_batch", "nmsm_set_window_bits", "nmsm_set_profiling", "nmsm_last_timing", "nmsm_bench_modmul",
     "nmsm_host_alloc", "nmsm_host_free", "nmsm_points_upload", "nmsm_points_free", "nmsm_msm_points", "nmsm_points_precompute", "nmsm_msm_points_submit", "nmsm_point_table_create", "nmsm_point_table_free",
     "nmsm_point_table_mul_batch", "nmsm_ntt", "nmsm_ntt_device", "nmsm_points_torsion_free",
-    "nmsm_ed25519_verify_batch", "nmsm_msm_submit", "nmsm_msm_collect", "nmsm_points_decode", "nmsm_msm_submit_partial",
+    "nmsm_ed25519_verify_batch", "nmsm_ed25519_verify_each", "nmsm_msm_submit", "nmsm_msm_collect", "nmsm_points_decode", "nmsm_msm_submit_partial",
     "nmsm_points_decode_ex", "nmsm_points_on_curve", "nmsm_set_window_groups", "nmsm_accs_normalize",
     "nmsm_dist_unique_id", "nmsm_dist_init", "nmsm_dist_info", "nmsm_dist_exchange_mode", "nmsm_msm_sharded", "nmsm_msm_sharded_submit",
     "nmsm_secp256k1_verify_batch", "nmsm_secp256k1_schnorr_verify_batch",
@@ -168,6 +168,8 @@ def load() -> ctypes.CDLL:
         lib.nmsm_ed25519_verify_batch.argtypes = [u8p, u8p, u8p, u8p, ctypes.c_uint64, u8p, ctypes.POINTER(ctypes.c_int),
                                                   ctypes.POINTER(ctypes.c_longlong)]
         lib.nmsm_ed25519_verify_batch.restype = ctypes.c_int
+        lib.nmsm_ed25519_verify_each.argtypes = [u8p, u8p, u8p, u8p, ctypes.c_uint64, ctypes.c_int, u8p]
+        lib.nmsm_ed25519_verify_each.restype = ctypes.c_int
         lib.nmsm_secp256k1_verify_batch.argtypes = [u8p, u8p, u8p, u8p, u8p, ctypes.c_uint64, ctypes.c_int, u8p]
         lib.nmsm_secp256k1_verify_batch.restype = ctypes.c_int
         lib.nmsm_secp256k1_schnorr_verify_batch.argtypes = [u8p, u8p, u8p, u8p, ctypes.c_uint64, u8p]
