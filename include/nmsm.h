@@ -23,6 +23,7 @@
  *   nmsm_ed25519_verify_batch <- ed25519.verify over a batch      edwards.ts:942-989
  *   nmsm_ed25519_verify_each <- ed25519.verify over a batch, one verdict per signature (ZIP-215 or strict)
  *   nmsm_secp256k1_verify_batch <- secp256k1.verify over a batch, one verdict per signature (weierstrass.ts ecdsa().verify)
+ *   nmsm_p256_verify_batch <- p256.verify over a batch, one verdict per signature (nist.ts; also EIP-7951 P256VERIFY)
  *   nmsm_secp256k1_schnorr_verify_batch <- schnorr.verify over a batch, one verdict per signature (secp256k1.ts, BIP340)
  *   nmsm_secp256k1_recover_batch <- secp256k1.recoverPublicKey over a batch (weierstrass.ts Signature.recoverPublicKey)
  *   nmsm_secp256k1_ecrecover_batch <- Ethereum's ecrecover precompile (0x01) over a batch
@@ -252,6 +253,18 @@ int nmsm_ed25519_verify_each(const uint8_t* sigs, const uint8_t* pubkeys, const 
 #define NMSM_ECDSA_LOW_S 2   /* s > n/2 verifies false (the reference's default lowS: true for secp256k1) */
 int nmsm_secp256k1_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint64_t* pk_off, const uint8_t* msgs,
                                 const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
+
+/* P-256 (secp256r1) ECDSA batch verification: out_ok[i] = p256.verify(sig_i, msg_i, pk_i, { prehash, lowS }) with
+ * format 'compact' (noble-curves nist.ts / weierstrass.ts ecdsa().verify), one independent verdict per signature.
+ * Arguments, rules, errors and flags as nmsm_secp256k1_verify_batch, on P-256 (y^2 = x^3 - 3x + b, SEC 2 §2.4.2):
+ * keys are 33-byte SEC1 compressed or 65-byte uncompressed P-256 points.  noble's p256 defaults are { prehash: true,
+ * lowS: false }, i.e. flags = NMSM_ECDSA_PREHASH, which is also what OpenSSL and the P256VERIFY precompile (EIP-7951,
+ * RIP-7212) check: a P256VERIFY input hash || r || s || qx || qy is this call with flags 0, the 32-byte hash as the
+ * message and 04 || qx || qy as the key.  The first call after nmsm_init builds the fixed-point table of the P-256 G
+ * (17 x 2^15 points, 36 MB), kept until nmsm_shutdown.  With profiling on, nmsm_last_timing reports
+ * k_p256_ecdsa_prepare in slot 0, k_p256_ecdsa_check in slot 1 and both in NMSM_T_TOTAL. */
+int nmsm_p256_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint64_t* pk_off, const uint8_t* msgs,
+                           const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
 
 /* secp256k1 BIP340 Schnorr batch verification (next-row f6): out_ok[i] = schnorr.verify(sig_i, msg_i, pk_i)
  * (noble-curves secp256k1.ts), one independent verdict per signature.

@@ -1,6 +1,7 @@
 // Wire-format decoding on the GPU (SURVEY §8 row f2): bytes -> canonical affine (x, y) in the C-ABI packing,
 // so callers can hand the encodings the reference's `fromBytes` consumes instead of bigints.
 //   secp256k1  SEC1 compressed, 33 B      /root/reference/src/abstract/weierstrass.ts:565-588 (pointFromBytes)
+//              (the same decoder serves P-256 ECDSA keys, ecdsa_verify.cuh)
 //   BLS12-381 G1  Zcash-flag compressed, 48 B   src/bls12-381.ts:377-468 (coder.decode, parseMask/validateMask)
 //   BLS12-381 G2  Zcash-flag compressed, 96 B   same coder over Fp2 (c1 || c0, bls12-381.ts:354-367,488-491), Fp2 sqrt tower.ts:476-498
 //   ed25519    RFC 8032 / ZIP-215, 32 B   src/abstract/edwards.ts:405-436  (ed25519_verify.cuh ed_decompress)
@@ -8,6 +9,7 @@
 // assertValidity (subgroup membership for cofactor > 1), which is a scalar multiplication of its own.
 #pragma once
 #include "ed25519_verify.cuh"
+#include "validate.cuh"
 
 namespace nmsm {
 
@@ -46,19 +48,28 @@ NMSM_HD void words_from_be_bytes(uint32_t* w, const uint8_t* b) {  // big-endian
   }
 }
 
-// status: 0 = invalid encoding, 1 = affine point written, 2 = point at infinity ((0,0) written)
-NMSM_HD int sec1_decode_secp256k1(const uint8_t* enc, uint32_t* out_xy) {
-  using F = Fp<FpSecp256k1>;
+// SEC1 compressed, 33 B: 02/03 || x, y = sqrt(x^3 + a x + b) with the prefix's parity, for a 256-bit prime field with
+// p = 3 (mod 4) (secp256k1, P-256).  status: 0 = invalid encoding, 1 = affine point written, 2 = point at infinity
+// ((0,0) written)
+template <class Cv>
+NMSM_HD int sec1_decode_compressed(const uint8_t* enc, uint32_t* out_xy) {
+  using F = typename Cv::G::Field;
   const uint8_t head = enc[0];
   if (head != 0x02 && head != 0x03) return 0;
   uint32_t xw[8];
   words_from_be_bytes<32>(xw, enc + 1);
   if (!F::canonical_in_range(xw)) return 0;  // Fp.fromBytes rejects x >= p
   const F x = F::from_canonical(xw);
-  F b;
-  for (int k = 0; k < 8; k++) b.v[k] = Secp256k1Consts::B_MONT(k);
+  F rhs;
+  if constexpr (Cv::ID == 0) {  // b from the generated Montgomery constant, not curve_b's conversion of 7
+    F b;
+    for (int k = 0; k < 8; k++) b.v[k] = Secp256k1Consts::B_MONT(k);
+    rhs = sqr(x) * x + b;
+  } else {
+    rhs = sw_rhs<Cv>(x);
+  }
   bool ok;
-  F y = fp_sqrt_3mod4<FpSecp256k1>(sqr(x) * x + b, ok);
+  F y = fp_sqrt_3mod4(rhs, ok);
   if (!ok) return 0;
   uint32_t yw[8];
   y.to_canonical(yw);
@@ -71,6 +82,9 @@ NMSM_HD int sec1_decode_secp256k1(const uint8_t* enc, uint32_t* out_xy) {
     out_xy[8 + k] = yw[k];
   }
   return 1;
+}
+NMSM_HD int sec1_decode_secp256k1(const uint8_t* enc, uint32_t* out_xy) {
+  return sec1_decode_compressed<CurveSecp256k1>(enc, out_xy);
 }
 
 NMSM_HD int zcash_decode_bls12_381_g1(const uint8_t* enc, uint32_t* out_xy) {

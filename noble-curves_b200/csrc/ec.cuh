@@ -4,9 +4,9 @@
 // coordinates (weierstrass.ts:793-880 RCB, edwards.ts:505-545 hwcd).  Results are only defined up
 // to the projective representative, so parity is on canonical affine (x, y) (test/point.test.ts:36-44).
 // Here:
-//   * short Weierstrass a = 0 (secp256k1, bn254 G1/G2, BLS12-381 G1/G2): XYZZ accumulators
+//   * short Weierstrass a = 0 (secp256k1, bn254 G1/G2, BLS12-381 G1/G2) and a = -3 (P-256): XYZZ accumulators
 //     (x = X/ZZ, y = Y/ZZZ, ZZ^3 = ZZZ^2; identity <=> ZZ == 0) with affine mixed addition
-//     madd-2008-s (8M+2S), add-2008-s (12M+2S), dbl-2008-s-1 (6M+3S for a=0), mdbl-2008-s-1.
+//     madd-2008-s (8M+2S), add-2008-s (12M+2S), dbl-2008-s-1 (6M+3S for a=0; 7M+2S for a=-3), mdbl-2008-s-1.
 //     The incomplete formulas are completed by explicit branches for P+P, P+(-P), O+P, P+O — all
 //     of which occur in the reference's own tests (point.test.ts:269,842-853).
 //   * twisted Edwards a = -1 (ed25519): extended coordinates with the unified, complete
@@ -75,11 +75,13 @@ struct Par4 {
 #endif
 
 // ------------------------------------------------------------------------------------------
-// Short Weierstrass, a = 0
+// Short Weierstrass y^2 = x^3 + A x + b, A = 0 or -3
 // ------------------------------------------------------------------------------------------
-template <class F>
+template <class F, int A = 0>
 struct SwXyzz {
+  static_assert(A == 0 || A == -3, "SwXyzz: a = 0 or a = -3");
   using Field = F;
+  static constexpr int CURVE_A = A;
   static constexpr int COORD_WORDS = F::LIMBS;
   static constexpr int IN_WORDS = 2 * F::LIMBS;   // canonical affine input (x, y)
   static constexpr int AFF_WORDS = 2 * F::LIMBS;  // prepared affine
@@ -116,27 +118,32 @@ struct SwXyzz {
   }
   NMSM_HD static Acc neg(const Acc& p) { return Acc{p.X, -p.Y, p.ZZ, p.ZZZ}; }
 
+  // M = 3 x^2 + a z^4 of the doublings, for zz = z^2: 3 x^2 (a = 0) or 3 (x - zz)(x + zz) (a = -3)
+  NMSM_HD static F dbl_m(const F& x, const F& zz) {
+    F xx;
+    if constexpr (A == 0) xx = sqr(x);
+    else xx = (x - zz) * (x + zz);
+    return nmsm::dbl(xx) + xx;
+  }
   // 2*(x, y) for an affine point: mdbl-2008-s-1
   NMSM_HD static Acc dbl_affine(const Affine& a) {
     F U = nmsm::dbl(a.y);
     F V = sqr(U);
     F W = U * V;
     F S = a.x * V;
-    F xx = sqr(a.x);
-    F M = nmsm::dbl(xx) + xx;
+    F M = dbl_m(a.x, F::one());
     F X3 = sqr(M) - nmsm::dbl(S);
     F Y3 = M * (S - X3) - W * a.y;
     return Acc{X3, Y3, V, W};  // y == 0 gives ZZ = 0 (identity), as it must for a 2-torsion point
   }
-  // dbl-2008-s-1, a = 0
+  // dbl-2008-s-1
   NMSM_HD static void dbl(Acc& p) {
     if (is_identity(p)) return;
     F U = nmsm::dbl(p.Y);
     F V = sqr(U);
     F W = U * V;
     F S = p.X * V;
-    F xx = sqr(p.X);
-    F M = nmsm::dbl(xx) + xx;
+    F M = dbl_m(p.X, p.ZZ);
     F X3 = sqr(M) - nmsm::dbl(S);
     F Y3 = M * (S - X3) - W * p.Y;
     p.ZZ = V * p.ZZ;
@@ -213,9 +220,11 @@ struct SwXyzz {
     p.Y = Y3;
   }
 #if defined(__CUDACC__)
-  // Warp-replicated versions of dbl / add (see Par4): 3 and 4 multiplication levels instead of 9 / 14.
+  // Warp-replicated versions of dbl / add (see Par4): 3 and 4 multiplication levels instead of 9 / 14.  a = 0 only:
+  // the MSM tail and k_mul_batch, which no a = -3 curve runs.
   template <bool FW>
   __device__ static void par_dbl(Acc& p) {
+    static_assert(A == 0, "par_dbl: a = 0 only");
     if (is_identity(p)) return;
     using P4 = Par4<F, FW>;
     F U = nmsm::dbl(p.Y);
@@ -526,6 +535,17 @@ struct CurveBls381G2Any {
   using Fn = Fn_bls12_381;
   static constexpr bool COFACTOR_ONE = false;
   static constexpr int ID = 7;
+};
+// NIST P-256 (secp256r1), a = -3: ECDSA verification only (inst_p256.cu).  No endomorphism, so scalar_mul_acc runs its
+// plain 4-bit windows and the fixed-point table of G has 17 levels.  ID 8 is reserved for P-256; no curve-id entry
+// point of the C ABI accepts it.
+struct CurveP256 {
+  static constexpr bool GLV = false;
+  static constexpr int GLV_KIND = 0;
+  using G = SwXyzz<Fp<FpP256>, -3>;
+  using Fn = Fn_p256;
+  static constexpr bool COFACTOR_ONE = true;
+  static constexpr int ID = 8;
 };
 
 }  // namespace nmsm

@@ -1,7 +1,7 @@
-// secp256k1 ECDSA batch verification (SURVEY §8 row f5): one independent verdict per signature.
+// ECDSA batch verification for secp256k1 (SURVEY §8 row f5) and P-256: one independent verdict per signature.
 //
 // The reference verifies one signature at a time: weierstrass.ts `ecdsa().verify` (noble-curves v2), with
-// format 'compact' and the options { prehash, lowS } (both default true for secp256k1):
+// format 'compact' and the options { prehash, lowS } (both default true for secp256k1; p256 defaults to lowS false):
 //   sig = r || s (64 B, big-endian); inside the reference's try (any failure = false):
 //   1 <= r, s < n;  P = Point.fromBytes(publicKey)  (33 B 02/03 + sqrt, or 65 B 04 + curve equation);
 //   lowS && s > n/2 -> false;  h = bits2int_modN(prehash ? sha256(msg) : msg)  (bits2int: > 8192 bytes throws);
@@ -10,17 +10,33 @@
 //   ecdsa_prepare_body  parse + range checks, lowS, key decode, SHA-256, bits2int mod n
 //   (kernel)            s^-1 through one warp-shared inversion per 32 signatures (msm.cuh warp_batch_inverse)
 //   ecdsa_store         u1, u2
-//   ecdsa_check_body    u1 G from the fixed-point table of G (table_mul_body), u2 Q (GLV scalar_mul_acc), complete
-//                       addition, and the x comparison in XYZZ coordinates without an inversion.
-// The two halves run as two kernels (inst_secp256k1.cu) so the SHA-256 / square-root state stays out of the scalar
-// multiplication's registers.  Bodies are host/device so tests/hostemu can run them.
+//   ecdsa_check_body    u1 G from the fixed-point table of G (table_mul_body), u2 Q (scalar_mul_acc: GLV on
+//                       secp256k1, plain windows on P-256), complete addition, and the x comparison in XYZZ
+//                       coordinates without an inversion.
+// The two halves run as two kernels (inst_secp256k1.cu, inst_p256.cu) so the SHA-256 / square-root state stays out of
+// the scalar multiplication's registers.  Bodies are host/device so tests/hostemu can run them.  They are templates on
+// the curve policy (CurveSecp256k1 by default, or CurveP256); what differs per curve is the group, the scalar modulus
+// n (EcdsaScalar) and the SEC1 key decoders.
 #pragma once
 #include "codec.cuh"
 #include "validate.cuh"
 
 namespace nmsm {
 
-using EcS = Fp<FnSecp256k1Mod>;
+// the scalar modulus n of each ECDSA curve (s^-1, u1, u2 mod n)
+template <class Cv>
+struct EcdsaScalar;
+template <>
+struct EcdsaScalar<CurveSecp256k1> {
+  using Mod = FnSecp256k1Mod;
+};
+template <>
+struct EcdsaScalar<CurveP256> {
+  using Mod = FnP256Mod;
+};
+template <class Cv>
+using EcdsaS = Fp<typename EcdsaScalar<Cv>::Mod>;
+using EcS = EcdsaS<CurveSecp256k1>;
 static constexpr int ECDSA_PREHASH = 1;  // include/nmsm.h NMSM_ECDSA_PREHASH
 static constexpr int ECDSA_LOW_S = 2;    // include/nmsm.h NMSM_ECDSA_LOW_S
 static constexpr uint64_t ECDSA_MAX_RAW_MSG = 8192;  // bits2int: "input is too large" above this many bytes
@@ -93,18 +109,22 @@ NMSM_HD void sha256(const uint8_t* msg, uint64_t len, uint8_t* out) {
 }
 
 // SEC1 uncompressed, 65 B: 04 || x || y, x < p, y < p, on the curve (weierstrass.ts pointFromBytes, `isValidXY`).
-// (0, 0) is rejected although point_on_curve accepts it as the identity encoding: 0 != 0^3 + 7.
-// status as sec1_decode_secp256k1: 0 = invalid, 1 = affine point written (canonical x, y words).
-NMSM_HD int sec1_decode_secp256k1_uncompressed(const uint8_t* enc, uint32_t* out_xy) {
+// (0, 0) is rejected although point_on_curve accepts it as the identity encoding: b != 0 on both curves.
+// status as sec1_decode_compressed: 0 = invalid, 1 = affine point written (canonical x, y words).
+template <class Cv>
+NMSM_HD int sec1_decode_uncompressed(const uint8_t* enc, uint32_t* out_xy) {
   if (enc[0] != 0x04) return 0;
   uint32_t xy[16];
   words_from_be_bytes<32>(xy, enc + 1);
   words_from_be_bytes<32>(xy + 8, enc + 33);
   uint32_t any = 0;
   for (int k = 0; k < 16; k++) any |= xy[k];
-  if (any == 0 || !point_on_curve<CurveSecp256k1>(xy)) return 0;
+  if (any == 0 || !point_on_curve<Cv>(xy)) return 0;
   for (int k = 0; k < 16; k++) out_xy[k] = xy[k];
   return 1;
+}
+NMSM_HD int sec1_decode_secp256k1_uncompressed(const uint8_t* enc, uint32_t* out_xy) {
+  return sec1_decode_uncompressed<CurveSecp256k1>(enc, out_xy);
 }
 
 NMSM_HD bool words8_nonzero(const uint32_t* a) {
@@ -113,9 +133,11 @@ NMSM_HD bool words8_nonzero(const uint32_t* a) {
   return t != 0;
 }
 // a > (n >> 1): the high-S test (Signature.hasHighS)
+template <class Cv = CurveSecp256k1>
 NMSM_HD bool ecdsa_high_s(const uint32_t* s) {
+  using Mod = typename EcdsaScalar<Cv>::Mod;
   for (int k = 7; k >= 0; k--) {
-    const uint32_t half = (FnSecp256k1Mod::P(k) >> 1) | (k < 7 ? FnSecp256k1Mod::P(k + 1) << 31 : 0u);
+    const uint32_t half = (Mod::P(k) >> 1) | (k < 7 ? Mod::P(k + 1) << 31 : 0u);
     if (s[k] != half) return s[k] > half;
   }
   return false;
@@ -123,7 +145,9 @@ NMSM_HD bool ecdsa_high_s(const uint32_t* s) {
 
 // h = bits2int_modN(prehash ? sha256(m) : m) for the message m[0..mlen): the big-endian integer of the first
 // min(len, 32) bytes, reduced mod n.  False for a raw message over ECDSA_MAX_RAW_MSG bytes (bits2int throws).
+template <class Cv = CurveSecp256k1>
 NMSM_HD bool ecdsa_msg_hash(const uint8_t* m, uint64_t mlen, int flags, uint32_t* h) {
+  using Mod = typename EcdsaScalar<Cv>::Mod;
   uint8_t digest[32];
   if (flags & ECDSA_PREHASH) {
     sha256(m, mlen, digest);
@@ -138,15 +162,16 @@ NMSM_HD bool ecdsa_msg_hash(const uint8_t* m, uint64_t mlen, int flags, uint32_t
     const int bit = 8 * (take - 1 - j);
     h[bit >> 5] |= (uint32_t)m[j] << (bit & 31);
   }
-  if (!EcS::canonical_in_range(h)) {  // h < 2^256 < 2n: one subtraction reduces it
-    h[0] = sub_cc(h[0], FnSecp256k1Mod::P(0));
-    for (int k = 1; k < 8; k++) h[k] = subc_cc(h[k], FnSecp256k1Mod::P(k));
+  if (!EcdsaS<Cv>::canonical_in_range(h)) {  // h < 2^256 < 2n: one subtraction reduces it
+    h[0] = sub_cc(h[0], Mod::P(0));
+    for (int k = 1; k < 8; k++) h[k] = subc_cc(h[k], Mod::P(k));
   }
   return true;
 }
 
 // Signature i: r, s, the public key Q (canonical affine words) and h = bits2int_modN(m).  False = the reference's
 // verify returns false before any scalar multiplication; the outputs are then unspecified.
+template <class Cv = CurveSecp256k1>
 NMSM_HD bool ecdsa_prepare_body(uint32_t i, const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off,
                                 const uint8_t* msgs, const uint64_t* msg_off, int flags, uint32_t* q_xy, uint32_t* r,
                                 uint32_t* s, uint32_t* h) {
@@ -154,56 +179,63 @@ NMSM_HD bool ecdsa_prepare_body(uint32_t i, const uint8_t* sigs, const uint8_t* 
   words_from_be_bytes<32>(r, sig);
   words_from_be_bytes<32>(s, sig + 32);
   // Signature.fromBytes: 1 <= r < n, 1 <= s < n;  then lowS
-  if (!words8_nonzero(r) || !EcS::canonical_in_range(r) || !words8_nonzero(s) || !EcS::canonical_in_range(s)) return false;
-  if ((flags & ECDSA_LOW_S) && ecdsa_high_s(s)) return false;
+  using S = EcdsaS<Cv>;
+  if (!words8_nonzero(r) || !S::canonical_in_range(r) || !words8_nonzero(s) || !S::canonical_in_range(s)) return false;
+  if ((flags & ECDSA_LOW_S) && ecdsa_high_s<Cv>(s)) return false;
   // Point.fromBytes
   const uint8_t* pk = pks + pk_off[i];
   const uint64_t pk_len = pk_off[i + 1] - pk_off[i];
   if (pk_len == 33) {
-    if (sec1_decode_secp256k1(pk, q_xy) != 1) return false;
+    if (sec1_decode_compressed<Cv>(pk, q_xy) != 1) return false;
   } else if (pk_len == 65) {
-    if (sec1_decode_secp256k1_uncompressed(pk, q_xy) != 1) return false;
+    if (sec1_decode_uncompressed<Cv>(pk, q_xy) != 1) return false;
   } else {
     return false;
   }
-  return ecdsa_msg_hash(msgs + msg_off[i], msg_off[i + 1] - msg_off[i], flags, h);
+  return ecdsa_msg_hash<Cv>(msgs + msg_off[i], msg_off[i + 1] - msg_off[i], flags, h);
 }
 
 // Given w = s^-1 (Montgomery form mod n): u1 = h w, u2 = r w, and the per-signature state k_ecdsa_check reads.
 // ok_out[i] carries the prepare verdict to the check, which overwrites it with the final one.
-NMSM_HD void ecdsa_store(uint32_t i, bool ok, const uint32_t* q_xy, const uint32_t* r, const uint32_t* h, const EcS& w,
-                         uint32_t* qs, uint32_t* u1s, uint32_t* u2s, uint32_t* rs, uint8_t* ok_out) {
+template <class Cv = CurveSecp256k1>
+NMSM_HD void ecdsa_store(uint32_t i, bool ok, const uint32_t* q_xy, const uint32_t* r, const uint32_t* h,
+                         const EcdsaS<Cv>& w, uint32_t* qs, uint32_t* u1s, uint32_t* u2s, uint32_t* rs, uint8_t* ok_out) {
+  using S = EcdsaS<Cv>;
   ok_out[i] = ok ? 1 : 0;
   if (!ok) return;
   uint32_t u1[8], u2[8];
-  (EcS::from_canonical(h) * w).to_canonical(u1);
-  (EcS::from_canonical(r) * w).to_canonical(u2);
+  (S::from_canonical(h) * w).to_canonical(u1);
+  (S::from_canonical(r) * w).to_canonical(u2);
   store_words<16>(qs + (size_t)i * 16, q_xy);
   store_words<8>(u1s + (size_t)i * 8, u1);
   store_words<8>(u2s + (size_t)i * 8, u2);
   store_words<8>(rs + (size_t)i * 8, r);
 }
 
-// serial statement of k_ecdsa_prepare (one inversion per signature instead of one per warp)
+// serial statement of k_ecdsa_prepare / k_p256_ecdsa_prepare (one inversion per signature instead of one per warp)
+template <class Cv = CurveSecp256k1>
 NMSM_HD void ecdsa_prepare_serial(uint32_t n, const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off,
                                   const uint8_t* msgs, const uint64_t* msg_off, int flags, uint32_t* qs, uint32_t* u1s,
                                   uint32_t* u2s, uint32_t* rs, uint8_t* ok_out) {
   for (uint32_t i = 0; i < n; i++) {
     uint32_t q[16], r[8], s[8], h[8];
-    const bool ok = ecdsa_prepare_body(i, sigs, pks, pk_off, msgs, msg_off, flags, q, r, s, h);
-    ecdsa_store(i, ok, q, r, h, ok ? inv(EcS::from_canonical(s)) : EcS::one(), qs, u1s, u2s, rs, ok_out);
+    const bool ok = ecdsa_prepare_body<Cv>(i, sigs, pks, pk_off, msgs, msg_off, flags, q, r, s, h);
+    using S = EcdsaS<Cv>;
+    ecdsa_store<Cv>(i, ok, q, r, h, ok ? inv(S::from_canonical(s)) : S::one(), qs, u1s, u2s, rs, ok_out);
   }
 }
 
 // R.x mod n == r for R = acc (XYZZ, x = X / ZZ), without an inversion: X == r ZZ, or, when r + n < p (R.x >= n is
-// possible because p - n ~ 2^128), X == (r + n) ZZ.  R = O (ZZ = 0) is false.
-NMSM_HD bool ecdsa_x_matches(const typename CurveSecp256k1::G::Acc& acc, const uint32_t* r) {
-  using F = CurveSecp256k1::G::Field;
-  if (CurveSecp256k1::G::is_identity(acc)) return false;
+// possible because p - n < 2^128 on both curves), X == (r + n) ZZ.  R = O (ZZ = 0) is false.
+template <class Cv = CurveSecp256k1>
+NMSM_HD bool ecdsa_x_matches(const typename Cv::G::Acc& acc, const uint32_t* r) {
+  using F = typename Cv::G::Field;
+  using Mod = typename EcdsaScalar<Cv>::Mod;
+  if (Cv::G::is_identity(acc)) return false;
   if (acc.X == F::from_canonical(r) * acc.ZZ) return true;  // r < n < p
   uint32_t rn[8];
-  rn[0] = add_cc(r[0], FnSecp256k1Mod::P(0));
-  for (int k = 1; k < 8; k++) rn[k] = addc_cc(r[k], FnSecp256k1Mod::P(k));
+  rn[0] = add_cc(r[0], Mod::P(0));
+  for (int k = 1; k < 8; k++) rn[k] = addc_cc(r[k], Mod::P(k));
   const uint32_t carry = addc(0, 0);
   if (carry || !F::canonical_in_range(rn)) return false;
   return acc.X == F::from_canonical(rn) * acc.ZZ;
@@ -211,26 +243,26 @@ NMSM_HD bool ecdsa_x_matches(const typename CurveSecp256k1::G::Acc& acc, const u
 
 // Signature i after ecdsa_store: R = u1 G + u2 Q, out_ok[i] = verdict.  tbl: the fixed-point table of G
 // (table_mul_body layout, BITS-bit digits; BITS is a parameter only so that tests/hostemu can use a small table).
-template <int BITS = PT_BITS>
+// u2 Q: GLV windows on secp256k1, plain 4-bit windows on P-256 (scalar_mul_acc).
+template <int BITS = PT_BITS, class Cv = CurveSecp256k1>
 NMSM_HD void ecdsa_check_body(uint32_t i, const uint32_t* tbl, const uint32_t* qs, const uint32_t* u1s,
                               const uint32_t* u2s, const uint32_t* rs, uint8_t* out_ok, unsigned int* err) {
-  using Cv = CurveSecp256k1;
-  using G = Cv::G;
+  using G = typename Cv::G;
   if (!out_ok[i]) return;
-  G::Acc acc;
+  typename G::Acc acc;
   table_mul_body<Cv, BITS>(i, tbl, u1s, 1, acc, err);  // u1 < n always; u1 = 0 (h = 0 mod n) gives O
   uint32_t q[16], u2[8], r[8];
   load_words<16>(q, qs + (size_t)i * 16);
   load_words<8>(u2, u2s + (size_t)i * 8);
   load_words<8>(r, rs + (size_t)i * 8);
   nl_add<G>(acc, scalar_mul_acc<Cv>(G::prepare(q), u2));  // complete: doubles when u1 G == u2 Q
-  out_ok[i] = ecdsa_x_matches(acc, r) ? 1 : 0;
+  out_ok[i] = ecdsa_x_matches<Cv>(acc, r) ? 1 : 0;
 }
 
-template <int BITS = PT_BITS>
+template <int BITS = PT_BITS, class Cv = CurveSecp256k1>
 NMSM_HD void ecdsa_check_serial(uint32_t n, const uint32_t* tbl, const uint32_t* qs, const uint32_t* u1s,
                                 const uint32_t* u2s, const uint32_t* rs, uint8_t* out_ok, unsigned int* err) {
-  for (uint32_t i = 0; i < n; i++) ecdsa_check_body<BITS>(i, tbl, qs, u1s, u2s, rs, out_ok, err);
+  for (uint32_t i = 0; i < n; i++) ecdsa_check_body<BITS, Cv>(i, tbl, qs, u1s, u2s, rs, out_ok, err);
 }
 
 }  // namespace nmsm

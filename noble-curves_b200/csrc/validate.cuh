@@ -15,11 +15,17 @@ NMSM_HD F field_from_small(uint32_t v) {
   return F::from_canonical(w);
 }
 
-// curve constant b of y^2 = x^3 + b (secp256k1.ts:48-56, bn254.ts:80-90,207-223, bls12-381.ts:134-148,321-345)
+// curve constant b of y^2 = x^3 + a x + b (secp256k1.ts:48-56, bn254.ts:80-90,207-223, bls12-381.ts:134-148,321-345;
+// P-256: SEC 2 §2.4.2)
 template <class Cv>
 NMSM_HD typename Cv::G::Field curve_b() {
   using F = typename Cv::G::Field;
   if constexpr (Cv::ID == 0) return field_from_small<F>(7);
+  else if constexpr (Cv::ID == 8) {
+    F b;
+    for (int k = 0; k < F::LIMBS; k++) b.v[k] = P256Consts::B_MONT(k);
+    return b;
+  }
   else if constexpr (Cv::ID == 2) return field_from_small<F>(3);
   else if constexpr (Cv::ID == 4 || Cv::ID == 6) return field_from_small<F>(4);
   else if constexpr (Cv::ID == 5 || Cv::ID == 7) {  // 4 * (1 + u)
@@ -30,6 +36,19 @@ NMSM_HD typename Cv::G::Field curve_b() {
     const uint32_t w[16] = {0x24a138e5u, 0x3267e6dcu, 0x59dbefa3u, 0xb5b4c5e5u, 0x1be06ac3u, 0x81be1899u, 0xceb8aaaeu, 0x2b149d40u,
                             0x85c315d2u, 0xe4a2bd06u, 0xe52d1852u, 0xa74fa084u, 0xeed8fdf4u, 0xcd2cafadu, 0x3af0fed4u, 0x009713b0u};
     return F::from_canonical(w);
+  }
+}
+
+// x^3 + a x + b, the right-hand side of the short Weierstrass equation (a = 0, or a = -3 as (x^2 - 3) x)
+template <class Cv>
+NMSM_HD typename Cv::G::Field sw_rhs(const typename Cv::G::Field& x) {
+  using F = typename Cv::G::Field;
+  if constexpr (Cv::G::CURVE_A == 0) {
+    return sqr(x) * x + curve_b<Cv>();
+  } else {
+    static_assert(Cv::G::CURVE_A == -3, "sw_rhs: a = 0 or a = -3");
+    const F three = nmsm::dbl(F::one()) + F::one();
+    return (sqr(x) - three) * x + curve_b<Cv>();
   }
 }
 
@@ -48,7 +67,7 @@ NMSM_HD int point_on_curve(const uint32_t* xy) {
     return (y2 - x2) == (F::one() + d * x2 * y2) ? 1 : 0;
   } else {
     if (x.is_zero() && y.is_zero()) return 1;
-    return sqr(y) == (sqr(x) * x + curve_b<Cv>()) ? 1 : 0;
+    return sqr(y) == sw_rhs<Cv>(x) ? 1 : 0;
   }
 }
 

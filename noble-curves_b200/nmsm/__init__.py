@@ -939,11 +939,7 @@ def _pack_offsets(items) -> bytes:
     return struct.pack("<%dQ" % len(offs), *offs)
 
 
-def ecdsa_verify_batch(signatures, messages, public_keys, prehash: bool = True, lowS: bool = True) -> List[bool]:
-    """Batch form of secp256k1.verify(sig, msg, publicKey, {prehash, lowS}) with format 'compact' (noble-curves
-    weierstrass.ts ecdsa().verify): one verdict per signature.  Raises where the reference throws before its `try`
-    (non-bytes arguments, a signature that is not 64 bytes) and for lists of different lengths; everything else
-    (r, s out of range, high s, an undecodable key, a raw message over 8192 bytes, R = O) is a False verdict."""
+def _check_ecdsa_args(signatures, messages, public_keys):
     n = len(signatures)
     if len(messages) != n or len(public_keys) != n:
         raise ValueError("signatures, messages and public keys must have equal length")
@@ -954,6 +950,15 @@ def ecdsa_verify_batch(signatures, messages, public_keys, prehash: bool = True, 
     for s in signatures:
         if len(s) != 64:
             raise ValueError('"compact signature" expected Uint8Array of length 64, got length=%d' % len(s))
+
+
+def ecdsa_verify_batch(signatures, messages, public_keys, prehash: bool = True, lowS: bool = True) -> List[bool]:
+    """Batch form of secp256k1.verify(sig, msg, publicKey, {prehash, lowS}) with format 'compact' (noble-curves
+    weierstrass.ts ecdsa().verify): one verdict per signature.  Raises where the reference throws before its `try`
+    (non-bytes arguments, a signature that is not 64 bytes) and for lists of different lengths; everything else
+    (r, s out of range, high s, an undecodable key, a raw message over 8192 bytes, R = O) is a False verdict."""
+    _check_ecdsa_args(signatures, messages, public_keys)
+    n = len(signatures)
     flags = (ECDSA_PREHASH if prehash else 0) | (ECDSA_LOW_S if lowS else 0)
     out = ecdsa_verify_batch_packed(b"".join(bytes(s) for s in signatures), b"".join(bytes(p) for p in public_keys),
                                     _pack_offsets(public_keys), b"".join(bytes(m) for m in messages),
@@ -989,6 +994,95 @@ def _secp256k1_verify(signature, message, publicKey, prehash: bool = True, lowS:
 
 
 secp256k1.verify = _secp256k1_verify
+
+
+def p256_ecdsa_verify_batch(signatures, messages, public_keys, prehash: bool = True, lowS: bool = False) -> List[bool]:
+    """Batch form of p256.verify(sig, msg, publicKey, {prehash, lowS}) with format 'compact' (noble-curves nist.ts,
+    weierstrass.ts ecdsa().verify): one verdict per signature.  The defaults are noble's for p256 (lowS false, as
+    OpenSSL).  Raises as ecdsa_verify_batch; everything else (r, s out of range, high s under lowS, an undecodable key,
+    a raw message over 8192 bytes, R = O) is a False verdict."""
+    _check_ecdsa_args(signatures, messages, public_keys)
+    flags = (ECDSA_PREHASH if prehash else 0) | (ECDSA_LOW_S if lowS else 0)
+    out = p256_ecdsa_verify_batch_packed(b"".join(bytes(s) for s in signatures),
+                                         b"".join(bytes(p) for p in public_keys), _pack_offsets(public_keys),
+                                         b"".join(bytes(m) for m in messages), _pack_offsets(messages),
+                                         len(signatures), flags)
+    return [b == 1 for b in out]
+
+
+def p256_ecdsa_verify_batch_packed(sigs: bytes, pks: bytes, pk_off: bytes, msgs: bytes, msg_off: bytes, n: int,
+                                   flags: int = ECDSA_PREHASH) -> bytes:
+    """The C-ABI call itself (nmsm_p256_verify_batch) on caller-packed arrays, laid out as for
+    ecdsa_verify_batch_packed.  Returns n verdict bytes (1 = valid)."""
+    if len(sigs) != 64 * n or len(pk_off) != 8 * (n + 1) or len(msg_off) != 8 * (n + 1):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    rc = lib.nmsm_p256_verify_batch(cp(sigs or b"\0"), cp(pks or b"\0"), cp(pk_off), cp(msgs or b"\0"), cp(msg_off), n,
+                                    flags, out)
+    try:
+        _lib.check(rc)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return out.raw[:n]
+
+
+def _p256_verify(signature, message, publicKey, prehash: bool = True, lowS: bool = False,
+                 format: str = "compact") -> bool:
+    """p256.verify for one signature (the batch entry point with n = 1)."""
+    if format != "compact":
+        raise NotImplementedError("signature format %r is not part of the accelerated path (compact only)" % (format,))
+    return p256_ecdsa_verify_batch([signature], [message], [publicKey], prehash=prehash, lowS=lowS)[0]
+
+
+# noble-curves' `p256` export (nist.ts; also `secp256r1`).  Verification only: P-256 is not an MSM curve and has no
+# Point class here, so it is not in CURVES.
+p256 = _NS(verify=_p256_verify)
+secp256r1 = p256
+
+P256VERIFY_INPUT_BYTES = 160  # EIP-7951 / RIP-7212: hash || r || s || qx || qy, 32 bytes each
+
+
+def p256verify_precompile_batch(inputs) -> List[bool]:
+    """Ethereum's P256VERIFY precompile (EIP-7951 on L1, RIP-7212 on rollups) over a batch: True where the precompile
+    returns the 32-byte word 1, False where it returns empty output.  `inputs` is a list of byte strings or one buffer
+    of n * 160 bytes.  An input that is not 160 bytes is False.  Each input runs as a P-256 ECDSA verification with
+    the 32-byte hash as the raw message (no prehash, no lowS) and the key 04 || qx || qy: that checks r, s in [1, n),
+    qx, qy < p, Q on the curve (which rejects (0, 0)), R != O and R.x mod n == r, the precompile's rules."""
+    import numpy as np
+
+    if isinstance(inputs, (bytes, bytearray, memoryview)):
+        buf = bytes(inputs)
+        if len(buf) % P256VERIFY_INPUT_BYTES:
+            raise ValueError("a packed P256VERIFY batch must be a multiple of 160 bytes, got %d" % len(buf))
+        items = np.frombuffer(buf, np.uint8).reshape(-1, P256VERIFY_INPUT_BYTES)
+        good = np.ones(len(items), bool)
+    else:
+        for x in inputs:
+            if not isinstance(x, (bytes, bytearray, memoryview)):
+                raise TypeError("P256VERIFY input expected bytes, got type=%s" % type(x).__name__)
+        good = np.array([len(x) == P256VERIFY_INPUT_BYTES for x in inputs], bool)
+        items = np.zeros((len(inputs), P256VERIFY_INPUT_BYTES), np.uint8)
+        for i, x in enumerate(inputs):
+            if good[i]:
+                items[i] = np.frombuffer(bytes(x), np.uint8)
+    idx = np.flatnonzero(good)
+    m = len(idx)
+    out = np.zeros(len(good), bool)
+    if m == 0:
+        return out.tolist()
+    sel = items[idx]
+    sigs = np.ascontiguousarray(sel[:, 32:96]).tobytes()
+    msgs = np.ascontiguousarray(sel[:, :32]).tobytes()
+    keys = np.empty((m, 65), np.uint8)
+    keys[:, 0] = 4
+    keys[:, 1:] = sel[:, 96:]
+    off = lambda w: (np.arange(m + 1, dtype="<u8") * w).tobytes()  # noqa: E731
+    res = p256_ecdsa_verify_batch_packed(sigs, keys.tobytes(), off(65), msgs, off(32), m, 0)
+    out[idx] = np.frombuffer(res, np.uint8) == 1
+    return out.tolist()
 
 
 def schnorr_verify_batch(signatures, messages, public_keys) -> List[bool]:
