@@ -31,6 +31,9 @@
  *   nmsm_bls12_381_hash_to_g2_batch <- bls12_381.G2.hashToCurve(msg, { DST }) over a batch (RFC 9380)
  *   nmsm_bls12_381_verify_msg_batch <- bls12_381.verify over a batch with the messages hashed on the GPU
  *   nmsm_bls12_381_aggregate_verify_batch <- FastAggregateVerify / bls.verifyBatch over a batch of checks
+ *   nmsm_bls12_381_hash_to_g1_batch <- bls12_381.G1.hashToCurve(msg, { DST }) over a batch (RFC 9380)
+ *   nmsm_bls12_381_short_verify_batch / _msg_batch <- bls12_381.verifyShortSignature over a batch (key in G2,
+ *                                                    signature in G1; messages hashed to G1 before or on the GPU)
  *   nmsm_ntt           <- FFT(rootsOfUnity(Fr, G), Fr).direct / .inverse   src/abstract/fft.ts:518-575
  *
  * Data formats (all little-endian, plain bytes, caller-owned):
@@ -394,6 +397,41 @@ int nmsm_bls12_381_verify_msg_batch(const uint8_t* sigs96, const uint8_t* pks48,
 int nmsm_bls12_381_aggregate_verify_batch(const uint8_t* sigs96, const uint64_t* group_off, uint64_t n_checks,
                                           const uint8_t* msgs, const uint64_t* msg_off, const uint8_t* keys_xy,
                                           const uint64_t* key_off, const uint8_t* dst, uint64_t dst_len,
+                                          uint8_t* out_ok);
+
+/* BLS12-381 hash to G1 (next-row f13): out_xy[i] = hash_to_curve(msg_i) on BLS12-381 G1, suite
+ * BLS12381G1_XMD:SHA-256_SSWU_RO_ (RFC 9380 §8.8.1; noble's bls12_381.G1.hashToCurve(msg, { DST })): expand_message_xmd
+ * with SHA-256 to 128 bytes, hash_to_field to two Fp elements, the simplified SWU map on the 11-isogenous curve and the
+ * isogeny, the sum of the two points, and cofactor clearing by h_eff = 1 - x.  Messages, tags (noble's default for
+ * short signatures is "BLS_SIG_BLS12381G1_XMD:SHA-256_SSWU_RO_NUL_"; a tag over 255 bytes is hashed as RFC 9380
+ * §5.3.3 says) and errors as for nmsm_bls12_381_hash_to_g2_batch.  out_xy: n x 96 B in the affine G1 packing (x, y,
+ * 48 B little-endian each, the NMSM_BLS12_381_G1 packing); the points are in G1; the identity, which only arises with
+ * negligible probability, is written as (0, 0).  With profiling on, nmsm_last_timing reports k_bls_hash_to_g1 in slot 0
+ * and in NMSM_T_TOTAL. */
+int nmsm_bls12_381_hash_to_g1_batch(const uint8_t* msgs, const uint64_t* msg_off, uint64_t n, const uint8_t* dst,
+                                    uint64_t dst_len, uint8_t* out_xy);
+
+/* BLS12-381 short-signature verification (next-row f13): out_ok[i] = bls12_381.verifyShortSignature(sig_i, H_i, pk_i),
+ * the IETF minimal-signature-size scheme (public key in G2, signature in G1), one independent verdict per signature.
+ * sigs48: n x 48 B Zcash-flag compressed G1 signatures; pks96: n x 96 B Zcash-flag compressed G2 keys; msg_pts: n x
+ * 96 B messages ALREADY HASHED to G1, in the affine G1 packing (nmsm_bls12_381_hash_to_g1_batch computes them;
+ * nmsm_bls12_381_short_verify_msg_batch takes the message bytes instead).
+ * out_ok[i] = 1 iff sig decodes, is not the identity and is in G1, pk decodes, is not the identity and is in G2, H is
+ * not the identity, and e(H, pk) e(sig, -G2) == 1.  Everything about a signature's or key's content is a 0 verdict,
+ * never an error.  H is only checked for range and curve: NMSM_ERR_POINT with nmsm_last_error_index = the smallest i
+ * whose H has a coordinate >= p or is off the curve.  NMSM_ERR_ARG for null pointers and n >= 2^30.  n == 0 writes
+ * nothing.  With profiling on, nmsm_last_timing reports k_bls_short_verify_prepare in slot 0, k_bls_miller in slot 1,
+ * k_bls_final in slot 2 and their sum in NMSM_T_TOTAL. */
+int nmsm_bls12_381_short_verify_batch(const uint8_t* sigs48, const uint8_t* pks96, const uint8_t* msg_pts, uint64_t n,
+                                      uint8_t* out_ok);
+
+/* nmsm_bls12_381_short_verify_batch with message i = msgs[msg_off[i], msg_off[i+1]) hashed to G1 on the GPU under dst,
+ * as nmsm_bls12_381_hash_to_g1_batch hashes it.  Every verdict rule of nmsm_bls12_381_short_verify_batch holds; the
+ * message points are in G1 by construction, so there is no message-point error.  NMSM_ERR_ARG as for
+ * nmsm_bls12_381_hash_to_g1_batch.  With profiling on, nmsm_last_timing reports k_bls_hash_to_g1 in slot 0,
+ * k_bls_short_verify_prepare in slot 1, k_bls_miller in slot 2, k_bls_final in slot 3 and their sum in NMSM_T_TOTAL. */
+int nmsm_bls12_381_short_verify_msg_batch(const uint8_t* sigs48, const uint8_t* pks96, const uint8_t* msgs,
+                                          const uint64_t* msg_off, uint64_t n, const uint8_t* dst, uint64_t dst_len,
                                           uint8_t* out_ok);
 
 /* Batched wire-format decoding on the GPU (next-row f2): encodings -> canonical affine points in the packing

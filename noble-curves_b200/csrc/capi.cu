@@ -908,6 +908,48 @@ int nmsm_bls12_381_verify_msg_batch(const uint8_t* sigs96, const uint8_t* pks48,
   return bls12_381_verify_msg_batch_impl(sigs96, pks48, msgs, msg_off, n, dst, dst_len, out_ok);
 }
 
+int nmsm_bls12_381_hash_to_g1_batch(const uint8_t* msgs, const uint64_t* msg_off, uint64_t n, const uint8_t* dst,
+                                    uint64_t dst_len, uint8_t* out_xy) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (!dst) return fail(NMSM_ERR_ARG, "null pointer");
+  if (dst_len == 0) return fail(NMSM_ERR_ARG, "dst must not be empty");
+  if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n must be < 2^30");  // before msg_off[n] is read
+  if (!msg_off || !out_xy) return fail(NMSM_ERR_ARG, "null pointer");
+  if (msg_off[n] && !msgs) return fail(NMSM_ERR_ARG, "null pointer");
+  return bls12_381_hash_to_g1_batch_impl(msgs, msg_off, n, dst, dst_len, out_xy);
+}
+
+int nmsm_bls12_381_short_verify_batch(const uint8_t* sigs48, const uint8_t* pks96, const uint8_t* msg_pts, uint64_t n,
+                                      uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (n == 0) return NMSM_OK;
+  if (!sigs48 || !pks96 || !msg_pts || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
+  return bls12_381_short_verify_batch_impl(sigs48, pks96, msg_pts, n, out_ok);
+}
+
+int nmsm_bls12_381_short_verify_msg_batch(const uint8_t* sigs48, const uint8_t* pks96, const uint8_t* msgs,
+                                          const uint64_t* msg_off, uint64_t n, const uint8_t* dst, uint64_t dst_len,
+                                          uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (!dst) return fail(NMSM_ERR_ARG, "null pointer");
+  if (dst_len == 0) return fail(NMSM_ERR_ARG, "dst must not be empty");
+  if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n must be < 2^30");  // before msg_off[n] is read
+  if (!sigs48 || !pks96 || !msg_off || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
+  if (msg_off[n] && !msgs) return fail(NMSM_ERR_ARG, "null pointer");
+  return bls12_381_short_verify_msg_batch_impl(sigs48, pks96, msgs, msg_off, n, dst, dst_len, out_ok);
+}
+
 int nmsm_bls12_381_aggregate_verify_batch(const uint8_t* sigs96, const uint64_t* group_off, uint64_t n_checks,
                                           const uint8_t* msgs, const uint64_t* msg_off, const uint8_t* keys_xy,
                                           const uint64_t* key_off, const uint8_t* dst, uint64_t dst_len,

@@ -249,6 +249,13 @@ int bls12_381_verify_msg_batch_impl(const uint8_t* sigs96, const uint8_t* pks48,
                                     uint8_t* out_ok);
 int bls12_381_hash_to_g2_batch_impl(const uint8_t* msgs, const uint64_t* msg_off, uint64_t n, const uint8_t* dst,
                                     uint64_t dst_len, uint8_t* out_xy);
+int bls12_381_hash_to_g1_batch_impl(const uint8_t* msgs, const uint64_t* msg_off, uint64_t n, const uint8_t* dst,
+                                    uint64_t dst_len, uint8_t* out_xy);
+int bls12_381_short_verify_batch_impl(const uint8_t* sigs48, const uint8_t* pks96, const uint8_t* msg_pts, uint64_t n,
+                                      uint8_t* out_ok);
+int bls12_381_short_verify_msg_batch_impl(const uint8_t* sigs48, const uint8_t* pks96, const uint8_t* msgs,
+                                          const uint64_t* msg_off, uint64_t n, const uint8_t* dst, uint64_t dst_len,
+                                          uint8_t* out_ok);
 int bls12_381_aggregate_verify_batch_impl(const uint8_t* sigs96, const uint64_t* group_off, uint64_t n_checks,
                                           const uint8_t* msgs, const uint64_t* msg_off, const uint8_t* keys_xy,
                                           const uint64_t* key_off, const uint8_t* dst, uint64_t dst_len,

@@ -1,9 +1,11 @@
-// BLS12-381 pairing checks, BLS signature verification (SURVEY §8 row f7, pairing.cuh), hash to G2 (f10,
-// hash_to_curve.cuh) and aggregate verification (f3, bls_aggregate.cuh): the kernels and the five C-ABI
-// implementations.  The chunked check driver is pairing_driver.cuh's (shared with bn254):
+// BLS12-381 pairing checks, BLS signature verification (SURVEY §8 row f7, pairing.cuh), hash to G2 (f10) and G1 (f13,
+// hash_to_curve.cuh), short-signature verification (f13) and aggregate verification (f3, bls_aggregate.cuh): the kernels
+// and the eight C-ABI implementations.  The chunked check driver is pairing_driver.cuh's (shared with bn254):
 //   k_bls_hash_to_g2      (hash, verify_msg, aggregate) one thread per message: RFC 9380 hash_to_curve, affine through
 //                         one inversion per warp
+//   k_bls_hash_to_g1      (hash to G1, short verify_msg) the same for G1
 //   k_bls_verify_prepare  (verify only) one thread per signature: decode, subgroup checks, the two pairs
+//   k_bls_short_verify_prepare  (short verify only) the same with sig in G1 and pk in G2
 //   k_bls_key_tiles       (aggregate only) one warp per tile of keys of one group: the partial key sums
 //   k_bls_key_groups      (aggregate only) one thread per group: its key sum S_g and the pair (S_g, H(m_g))
 //   k_bls_agg_prepare     (aggregate only) one thread per check: signature decode and subgroup check, the pair (-G1, sig)
@@ -49,6 +51,25 @@ k_bls_hash_to_g2(uint32_t n, const uint8_t* __restrict__ msgs, const uint64_t* _
   if (i < n) q = h2c_hash_body(i, msgs, msg_off, dst, dlen);
   const H2cF2 zi = warp_batch_inverse(H2cG::inv_target(q));
   if (i < n) h2c_store(i, q, zi, out);
+}
+
+__global__ void __launch_bounds__(PAIRING_BLOCK)
+k_bls_short_verify_prepare(uint32_t n, const uint8_t* __restrict__ sigs, const uint8_t* __restrict__ pks,
+                           const uint32_t* __restrict__ msg_pts, uint32_t* __restrict__ g1, uint32_t* __restrict__ g2,
+                           uint8_t* __restrict__ pre_ok, unsigned int* err) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) bls_short_verify_prepare_body(i, sigs, pks, msg_pts, g1, g2, pre_ok, err);
+}
+
+// Lanes past n feed the identity, whose inversion target is 1, to the warp-shared inversion.
+__global__ void __launch_bounds__(128)
+k_bls_hash_to_g1(uint32_t n, const uint8_t* __restrict__ msgs, const uint64_t* __restrict__ msg_off,
+                 const uint8_t* __restrict__ dst, uint32_t dlen, uint32_t* __restrict__ out) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  H2cG1::Acc q = H2cG1::identity();
+  if (i < n) q = h2c_hash_body_g1(i, msgs, msg_off, dst, dlen);
+  const H2cF zi = warp_batch_inverse(H2cG1::inv_target(q));
+  if (i < n) h2c_store_g1(i, q, zi, out);
 }
 
 // one warp per tile (4 per block): lane sums, then a shuffle tree whose lane 0 writes the partial and the bad flag
@@ -124,8 +145,10 @@ BlsMessages bls_messages(const uint8_t* msgs, const uint64_t* msg_off, const uin
 // workspace bytes of bls_hash_launch for n messages
 uint64_t bls_hash_bytes(const BlsMessages& m, uint64_t n) { return al256(m.msg_off[n] + 16) + al256(8 * (n + 1)) + 256; }
 
-// uploads the messages, offsets and tag to ws (bls_hash_bytes) and runs k_bls_hash_to_g2 into d_out (timing slot 0)
-int bls_hash_launch(Context& X, Slot& C, const BlsMessages& m, uint64_t n, uint8_t* ws, uint32_t* d_out) {
+// uploads the messages, offsets and tag to ws (bls_hash_bytes) and runs k_bls_hash_to_g2, or k_bls_hash_to_g1 when g1,
+// into d_out (timing slot 0)
+int bls_hash_launch(Context& X, Slot& C, const BlsMessages& m, uint64_t n, uint8_t* ws, uint32_t* d_out,
+                    bool g1 = false) {
   cudaStream_t st = C.stream;
   const uint64_t msg_bytes = m.msg_off[n], o_mo = al256(msg_bytes + 16), o_dst = o_mo + al256(8 * (n + 1));
   if (msg_bytes)
@@ -133,21 +156,23 @@ int bls_hash_launch(Context& X, Slot& C, const BlsMessages& m, uint64_t n, uint8
   if (int r = h2d_any(ws + o_mo, m.msg_off, 8 * (n + 1), st)) return r;
   if (int r = h2d_any(ws + o_dst, m.dst, m.dlen, st)) return r;
   return pairing_launch(X, C, 0, [&] {
-    k_bls_hash_to_g2<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, ws, (const uint64_t*)(ws + o_mo), ws + o_dst, m.dlen,
-                                                   d_out);
+    (g1 ? k_bls_hash_to_g1 : k_bls_hash_to_g2)<<<cdiv(n, 128), 128, 0, st>>>(
+        (uint32_t)n, ws, (const uint64_t*)(ws + o_mo), ws + o_dst, m.dlen, d_out);
   });
 }
 
 // nmsm_bls12_381_verify_batch (msg_pts on the host) and nmsm_bls12_381_verify_msg_batch (hm: the messages, hashed
-// into the same workspace by k_bls_hash_to_g2, which shifts the other kernels' timing slots by one)
-int bls_verify_impl(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* msg_pts, const BlsMessages* hm,
-                    uint64_t n, uint8_t* out_ok) {
+// into the same workspace by k_bls_hash_to_g2, which shifts the other kernels' timing slots by one); with short_sigs,
+// the short-signature forms (48-byte G1 signatures, 96-byte G2 keys, G1 message points and k_bls_hash_to_g1)
+int bls_verify_impl(const uint8_t* sigs, const uint8_t* pks, const uint8_t* msg_pts, const BlsMessages* hm,
+                    uint64_t n, uint8_t* out_ok, bool short_sigs = false) {
   Context& X = g_ctx;
   Slot& C = X.slot[0];
   if (n == 0) return NMSM_OK;
   if (n >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n must be < 2^30");
   if (X.profiling) memset(X.last_ms, 0, sizeof(X.last_ms));
-  const uint64_t o_sig = 0, o_pk = o_sig + al256(96 * n), o_h = o_pk + al256(48 * n), o_g1 = o_h + al256(192 * n),
+  const uint64_t sig_b = short_sigs ? 48 : 96, pk_b = short_sigs ? 96 : 48, h_b = short_sigs ? 96 : 192;
+  const uint64_t o_sig = 0, o_pk = o_sig + al256(sig_b * n), o_h = o_pk + al256(pk_b * n), o_g1 = o_h + al256(h_b * n),
                  o_g2 = o_g1 + al256(192 * n), o_pre = o_g2 + al256(384 * n),
                  o_w = o_pre + al256(n), o_ok = o_w + al256(pairing_workspace_bytes<BlsPairing>()),
                  o_misc = o_ok + al256(n), o_hash = o_misc + 256, bytes = o_hash + (hm ? bls_hash_bytes(*hm, n) : 0);
@@ -155,11 +180,11 @@ int bls_verify_impl(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* 
   uint8_t* base = (uint8_t*)X.ed_scratch.p;
   cudaStream_t st = C.stream;
   const int s0 = hm ? 1 : 0;
-  if (int r = h2d_any(base + o_sig, sigs96, 96 * n, st)) return r;
-  if (int r = h2d_any(base + o_pk, pks48, 48 * n, st)) return r;
+  if (int r = h2d_any(base + o_sig, sigs, sig_b * n, st)) return r;
+  if (int r = h2d_any(base + o_pk, pks, pk_b * n, st)) return r;
   if (hm) {
-    if (int r = bls_hash_launch(X, C, *hm, n, base + o_hash, (uint32_t*)(base + o_h))) return r;
-  } else if (int r = h2d_any(base + o_h, msg_pts, 192 * n, st)) {
+    if (int r = bls_hash_launch(X, C, *hm, n, base + o_hash, (uint32_t*)(base + o_h), short_sigs)) return r;
+  } else if (int r = h2d_any(base + o_h, msg_pts, h_b * n, st)) {
     return r;
   }
   unsigned int* d_err = (unsigned int*)(base + o_misc);
@@ -167,7 +192,8 @@ int bls_verify_impl(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* 
   uint8_t *d_pre = base + o_pre, *d_ok = base + o_ok;
   CK(cudaMemsetAsync(d_err, 0xff, 16, st));
   if (int r = pairing_launch(X, C, s0, [&] {
-        k_bls_verify_prepare<<<cdiv(n, PAIRING_BLOCK), PAIRING_BLOCK, 0, st>>>(
+        (short_sigs ? k_bls_short_verify_prepare : k_bls_verify_prepare)<<<cdiv(n, PAIRING_BLOCK), PAIRING_BLOCK, 0,
+                                                                           st>>>(
             (uint32_t)n, base + o_sig, base + o_pk, (const uint32_t*)(base + o_h), d_g1, d_g2, d_pre, d_err);
       }))
     return r;
@@ -177,10 +203,10 @@ int bls_verify_impl(const uint8_t* sigs96, const uint8_t* pks48, const uint8_t* 
   unsigned int err[4];
   CK(cudaMemcpyAsync(err, d_err, 16, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  if (err[0] != 0xffffffffu)  // hashed messages are on the twist by construction
+  if (err[0] != 0xffffffffu)  // hashed messages are on their curve by construction
     return fail(hm ? NMSM_ERR_CUDA : NMSM_ERR_POINT,
                 (hm ? "internal error: hashed message point " : "message point ") + std::to_string(err[0]) +
-                    " is out of range or not on the twist",
+                    (short_sigs ? " is out of range or not on the curve" : " is out of range or not on the twist"),
                 err[0]);
   if (err[2] != 0xffffffffu || err[3] != 0xffffffffu)  // prepare only emits valid or identity pairs
     return fail(NMSM_ERR_CUDA, "internal error: a prepared pair failed validation");
@@ -305,8 +331,10 @@ int bls12_381_verify_msg_batch_impl(const uint8_t* sigs96, const uint8_t* pks48,
   return bls_verify_impl(sigs96, pks48, nullptr, &hm, n, out_ok);
 }
 
-int bls12_381_hash_to_g2_batch_impl(const uint8_t* msgs, const uint64_t* msg_off, uint64_t n, const uint8_t* dst,
-                                    uint64_t dst_len, uint8_t* out_xy) {
+namespace {
+// nmsm_bls12_381_hash_to_g2_batch, or nmsm_bls12_381_hash_to_g1_batch when g1 (96-byte instead of 192-byte points)
+int bls_hash_impl(const uint8_t* msgs, const uint64_t* msg_off, uint64_t n, const uint8_t* dst, uint64_t dst_len,
+                  uint8_t* out_xy, bool g1) {
   Context& X = g_ctx;
   Slot& C = X.slot[0];
   if (n == 0) return NMSM_OK;
@@ -315,13 +343,40 @@ int bls12_381_hash_to_g2_batch_impl(const uint8_t* msgs, const uint64_t* msg_off
   std::vector<uint8_t> tag;
   const BlsMessages hm = bls_messages(msgs, msg_off, dst, dst_len, tag);
   if (X.profiling) memset(X.last_ms, 0, sizeof(X.last_ms));
-  const uint64_t o_out = 0, o_hash = al256(192 * n), bytes = o_hash + bls_hash_bytes(hm, n);
+  const uint64_t pt_b = g1 ? 96 : 192, o_out = 0, o_hash = al256(pt_b * n), bytes = o_hash + bls_hash_bytes(hm, n);
   CK(X.ed_scratch.ensure(bytes));
   uint8_t* base = (uint8_t*)X.ed_scratch.p;
-  if (int r = bls_hash_launch(X, C, hm, n, base + o_hash, (uint32_t*)(base + o_out))) return r;
-  CK(cudaMemcpyAsync(out_xy, base + o_out, 192 * n, cudaMemcpyDeviceToHost, C.stream));
+  if (int r = bls_hash_launch(X, C, hm, n, base + o_hash, (uint32_t*)(base + o_out), g1)) return r;
+  CK(cudaMemcpyAsync(out_xy, base + o_out, pt_b * n, cudaMemcpyDeviceToHost, C.stream));
   CK(cudaStreamSynchronize(C.stream));
   return NMSM_OK;
+}
+}  // namespace
+
+int bls12_381_hash_to_g2_batch_impl(const uint8_t* msgs, const uint64_t* msg_off, uint64_t n, const uint8_t* dst,
+                                    uint64_t dst_len, uint8_t* out_xy) {
+  return bls_hash_impl(msgs, msg_off, n, dst, dst_len, out_xy, false);
+}
+
+int bls12_381_hash_to_g1_batch_impl(const uint8_t* msgs, const uint64_t* msg_off, uint64_t n, const uint8_t* dst,
+                                    uint64_t dst_len, uint8_t* out_xy) {
+  return bls_hash_impl(msgs, msg_off, n, dst, dst_len, out_xy, true);
+}
+
+int bls12_381_short_verify_batch_impl(const uint8_t* sigs48, const uint8_t* pks96, const uint8_t* msg_pts, uint64_t n,
+                                      uint8_t* out_ok) {
+  return bls_verify_impl(sigs48, pks96, msg_pts, nullptr, n, out_ok, true);
+}
+
+int bls12_381_short_verify_msg_batch_impl(const uint8_t* sigs48, const uint8_t* pks96, const uint8_t* msgs,
+                                          const uint64_t* msg_off, uint64_t n, const uint8_t* dst, uint64_t dst_len,
+                                          uint8_t* out_ok) {
+  if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n must be < 2^30");
+  if (int r = check_offsets(msg_off, "msg_off", n)) return r;
+  std::vector<uint8_t> tag;
+  const BlsMessages hm = bls_messages(msgs, msg_off, dst, dst_len, tag);
+  return bls_verify_impl(sigs48, pks96, nullptr, &hm, n, out_ok, true);
 }
 
 }  // namespace nmsm

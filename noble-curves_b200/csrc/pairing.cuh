@@ -4,6 +4,7 @@
 // question asked of the GPU is always "is this product of pairings 1", one verdict per check:
 //   check j:  prod_{i in [off[j], off[j+1])} e(P_i, Q_i) == 1,   P_i in E(Fp), Q_i on the twist E'(Fp2): y^2 = x^3 + 4 xi
 //   verify:   e(pk, H) e(-G1, sig) == 1                            (long signatures: pk in G1, sig and H = H(m) in G2)
+//   short:    e(H, pk) e(sig, -G2) == 1                            (short signatures: pk in G2, sig and H = H(m) in G1)
 //
 // Miller loop: f_{|x|,Q}(P) over the bits of |x| = 0xd201000000010000 (x < 0): 63 doubling steps and 5 addition
 // steps.  T runs in homogeneous projective coordinates on the twist (Costello-Lange-Naehrig doubling, mixed addition
@@ -170,6 +171,51 @@ NMSM_HD void bls_verify_prepare_body(uint32_t i, const uint8_t* sigs96, const ui
   for (int k = 0; k < 48; k++) {
     q0[k] = ok ? h[k] : 0u;
     q0[48 + k] = ok ? sig[k] : 0u;
+  }
+  pre_ok[i] = ok ? 1 : 0;
+}
+
+// the generator of G2, negated: (Gx, -Gy) canonical in the G2 packing (x.c0, x.c1, y.c0, y.c1)
+NMSM_HD uint32_t bls_neg_g2(int k) {
+  constexpr uint32_t W[48] = {0xc121bdb8u, 0xd48056c8u, 0xa805bbefu, 0x0bac0326u, 0x7ae3d177u, 0xb4510b64u,
+                              0xfa403b02u, 0xc6e47ad4u, 0x2dc51051u, 0x26080527u, 0xf08f0a91u, 0x024aa2b2u,
+                              0x5d042b7eu, 0xe5ac7d05u, 0x13945d57u, 0x334cf112u, 0xdc7f5049u, 0xb5da61bbu,
+                              0x9920b61au, 0x596bd0d0u, 0x88274f65u, 0x7dacd3a0u, 0x52719f60u, 0x13e02b60u,
+                              0xf74782aau, 0xd86bab79u, 0x75a75d75u, 0x8c713632u, 0xa55024f7u, 0xf9ee3837u,
+                              0x66c73f17u, 0xb679afdau, 0x691d77bcu, 0xbe51d9efu, 0xc7027888u, 0x0d1b3cc2u,
+                              0x0fa030edu, 0x0f55f8a0u, 0x5467e25eu, 0xdf74f2d7u, 0x9f825c78u, 0x40bc3ff5u,
+                              0x6dddaf10u, 0x99392306u, 0x1789213du, 0x186ed506u, 0x0ad8b1ceu, 0x13fa4d4au};
+  return W[k];
+}
+
+// k_bls_short_verify_prepare, signature i (short signatures, bls_verify_prepare_body with the groups swapped): decode
+// sig (48 B, G1) and pk (96 B, G2), reject identities and points outside the subgroups, range- and curve-check the G1
+// point H (a caller error: err[0] = smallest bad index).  Writes the pairs 2i = (H, pk) and 2i + 1 = (sig, -G2), or two
+// identity pairs when the signature is rejected, and pre_ok[i].
+NMSM_HD void bls_short_verify_prepare_body(uint32_t i, const uint8_t* sigs48, const uint8_t* pks96,
+                                           const uint32_t* msg_pts, uint32_t* g1, uint32_t* g2, uint8_t* pre_ok,
+                                           unsigned int* err) {
+  uint32_t sig[24], pk[48], h[24];
+  load_words<24>(h, msg_pts + (size_t)i * 24);
+  bool ok = true;
+  if (!point_on_curve<CurveBls381G1Any>(h)) {
+    atomic_min_u32(&err[0], i);
+    ok = false;
+  }
+  ok = ok && !words_zero(h, 24);
+  ok = ok && zcash_decode_bls12_381_g1(sigs48 + (size_t)i * 48, sig) == 1;
+  ok = ok && zcash_decode_bls12_381_g2(pks96 + (size_t)i * 96, pk) == 1;
+  ok = ok && bls_in_subgroup<CurveBls381G1Any>(sig);
+  ok = ok && bls_in_subgroup<CurveBls381G2Any>(pk);
+  uint32_t* p0 = g1 + (size_t)i * 48;
+  uint32_t* q0 = g2 + (size_t)i * 96;
+  for (int k = 0; k < 24; k++) {
+    p0[k] = ok ? h[k] : 0u;
+    p0[24 + k] = ok ? sig[k] : 0u;
+  }
+  for (int k = 0; k < 48; k++) {
+    q0[k] = ok ? pk[k] : 0u;
+    q0[48 + k] = ok ? bls_neg_g2(k) : 0u;
   }
   pre_ok[i] = ok ? 1 : 0;
 }

@@ -1601,6 +1601,161 @@ def _bls_verify_batch(signature, messages, publicKeys) -> bool:
 bls12_381.verifyBatch = _bls_verify_batch
 
 
+# ---- BLS12-381 hash to G1 and short signatures (include/nmsm.h nmsm_bls12_381_hash_to_g1_batch,
+# nmsm_bls12_381_short_verify_batch, nmsm_bls12_381_short_verify_msg_batch) ------------------------------------------
+DST_G1_NUL = b"BLS_SIG_BLS12381G1_XMD:SHA-256_SSWU_RO_NUL_"  # noble's default tag for short signatures
+DST_G1_POP = b"BLS_SIG_BLS12381G1_XMD:SHA-256_SSWU_RO_POP_"  # proof-of-possession scheme, minimal-signature-size
+
+
+def bls_hash_to_g1_batch(messages, dst=DST_G1_NUL) -> List:
+    """Batch form of bls12_381.G1.hashToCurve(msg, { DST }) (RFC 9380 suite BLS12381G1_XMD:SHA-256_SSWU_RO_): one
+    bls12_381.G1.Point per message, each in G1.  Messages are bytes of any length; the tag is non-empty bytes (or str),
+    one tag for the whole batch."""
+    msgs, dst = _h2c_args(messages, dst)
+    if not msgs:
+        return []
+    xy = bls_hash_to_g1_batch_packed(b"".join(msgs), _pack_offsets(msgs), len(msgs), dst)
+    G1 = bls12_381.G1.Point
+    out = []
+    for k in range(len(msgs)):
+        b = xy[96 * k:96 * k + 96]
+        out.append(G1.from_packed(b, not any(b), valid=True))
+    return out
+
+
+def bls_hash_to_g1_batch_packed(msgs: bytes, msg_off: bytes, n: int, dst: bytes) -> bytes:
+    """The C-ABI call itself (nmsm_bls12_381_hash_to_g1_batch): the concatenated messages with n+1 little-endian u64
+    offsets and the tag.  Returns n*96 bytes of affine G1 points; raises NmsmError (with .code) on an error."""
+    if len(msg_off) != 8 * (n + 1):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(96 * n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    _lib.check(lib.nmsm_bls12_381_hash_to_g1_batch(cp(msgs or b"\0"), cp(msg_off), n, cp(dst or b"\0"), len(dst), out))
+    return out.raw[:96 * n]
+
+
+def _g1_hash_to_curve(msg, options=None):
+    """bls12_381.G1.hashToCurve(msg, { DST }) for one message (the batch entry point with n = 1); the default tag is
+    noble's BLS_SIG_BLS12381G1_XMD:SHA-256_SSWU_RO_NUL_."""
+    dst = DST_G1_NUL
+    if options is not None:
+        if not isinstance(options, dict):
+            raise TypeError("options expected dict, got type=%s" % type(options).__name__)
+        dst = options.get("DST", DST_G1_NUL)
+    return bls_hash_to_g1_batch([msg], dst)[0]
+
+
+bls12_381.G1.hashToCurve = _g1_hash_to_curve
+
+
+def _bls_short_sigs_and_keys(signatures, public_keys):
+    """the packed signature and key arguments of the short-signature entry points: 48-byte and 96-byte Zcash-flag
+    compressed encodings, or Points (encoded first)"""
+    G1, G2 = bls12_381.G1.Point, bls12_381.G2.Point
+    sigs, pks = [], []
+    for s in signatures:
+        if isinstance(s, G1):
+            s = s.toBytes(True)
+        if not isinstance(s, (bytes, bytearray, memoryview)):
+            raise TypeError('"signature" expected Uint8Array or G1 Point, got type=%s' % type(s).__name__)
+        if len(s) != 48:
+            raise ValueError('"signature" expected Uint8Array of length 48, got length=%d' % len(s))
+        sigs.append(bytes(s))
+    for k in public_keys:
+        if isinstance(k, G2):
+            k = _bls_g2_compress(k)
+        if not isinstance(k, (bytes, bytearray, memoryview)):
+            raise TypeError('"publicKey" expected Uint8Array or G2 Point, got type=%s' % type(k).__name__)
+        if len(k) != 96:
+            raise ValueError('"publicKey" expected Uint8Array of length 96, got length=%d' % len(k))
+        pks.append(bytes(k))
+    return b"".join(sigs), b"".join(pks)
+
+
+def bls_short_verify_batch(signatures, message_points, public_keys) -> List[bool]:
+    """Batch form of bls12_381.verifyShortSignature(signature, message, publicKey) (public key in G2, signature in G1):
+    one verdict per signature.  Signatures are 48-byte and keys 96-byte Zcash-flag compressed encodings, or Points
+    (encoded first).  Messages are already hashed to G1 (bls12_381.G1.Point; bls_short_verify_messages_batch takes
+    bytes).  A signature or key that does not decode, is the identity or lies outside its subgroup is a False verdict;
+    a message point off the curve raises ValueError."""
+    n = len(signatures)
+    if len(message_points) != n or len(public_keys) != n:
+        raise ValueError("signatures, messages and public keys must have equal length")
+    sigs, pks = _bls_short_sigs_and_keys(signatures, public_keys)
+    G1 = bls12_381.G1.Point
+    for m in message_points:
+        if not isinstance(m, G1):
+            raise TypeError('"message" expected bls12_381.G1.Point (bls_short_verify_messages_batch takes bytes), got '
+                            'type=%s' % type(m).__name__)
+    if n == 0:
+        return []
+    try:
+        out = bls_short_verify_batch_packed(sigs, pks, _pack_points(message_points), n)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return [b == 1 for b in out]
+
+
+def bls_short_verify_batch_packed(sigs48: bytes, pks96: bytes, msg_pts: bytes, n: int) -> bytes:
+    """The C-ABI call itself (nmsm_bls12_381_short_verify_batch): n*48 signature bytes, n*96 key bytes and n*96 bytes
+    of affine G1 message points.  Returns n verdict bytes; raises NmsmError (with .code and .index) on an error."""
+    if len(sigs48) != 48 * n or len(pks96) != 96 * n or len(msg_pts) != 96 * n:
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    _lib.check(lib.nmsm_bls12_381_short_verify_batch(cp(sigs48 or b"\0"), cp(pks96 or b"\0"), cp(msg_pts or b"\0"), n,
+                                                     out))
+    return out.raw[:n]
+
+
+def bls_short_verify_messages_batch(signatures, messages, public_keys, dst=DST_G1_NUL) -> List[bool]:
+    """bls_short_verify_batch with message bytes, hashed to G1 on the GPU under dst in the same call: verdict i is
+    bls12_381.verifyShortSignature(signature_i, G1.hashToCurve(message_i, { DST }), publicKey_i)."""
+    n = len(signatures)
+    if len(messages) != n or len(public_keys) != n:
+        raise ValueError("signatures, messages and public keys must have equal length")
+    msgs, dst = _h2c_args(messages, dst)
+    sigs, pks = _bls_short_sigs_and_keys(signatures, public_keys)
+    if n == 0:
+        return []
+    try:
+        out = bls_short_verify_messages_batch_packed(sigs, pks, b"".join(msgs), _pack_offsets(msgs), n, dst)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return [b == 1 for b in out]
+
+
+def bls_short_verify_messages_batch_packed(sigs48: bytes, pks96: bytes, msgs: bytes, msg_off: bytes, n: int,
+                                           dst: bytes) -> bytes:
+    """The C-ABI call itself (nmsm_bls12_381_short_verify_msg_batch): n*48 signature bytes, n*96 key bytes, the
+    concatenated messages with n+1 little-endian u64 offsets and the tag.  Returns n verdict bytes; raises NmsmError on
+    an error."""
+    if len(sigs48) != 48 * n or len(pks96) != 96 * n or len(msg_off) != 8 * (n + 1):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    _lib.check(lib.nmsm_bls12_381_short_verify_msg_batch(cp(sigs48 or b"\0"), cp(pks96 or b"\0"), cp(msgs or b"\0"),
+                                                         cp(msg_off), n, cp(dst or b"\0"), len(dst), out))
+    return out.raw[:n]
+
+
+def _bls_verify_short_signature(signature, message, publicKey) -> bool:
+    """bls12_381.verifyShortSignature for one signature: a bytes message is hashed to G1 under DST_G1_NUL, as noble
+    does; a bls12_381.G1.Point is taken as already hashed."""
+    if isinstance(message, (bytes, bytearray, memoryview)):
+        return bls_short_verify_messages_batch([signature], [message], [publicKey], DST_G1_NUL)[0]
+    return bls_short_verify_batch([signature], [message], [publicKey])[0]
+
+
+bls12_381.verifyShortSignature = _bls_verify_short_signature
+
+
 # ---- bn254 pairing checks (include/nmsm.h nmsm_bn254_pairing_check_batch) and EIP-197 ecPairing ---------------------
 def bn254_pairing_check_batch(checks) -> List[bool]:
     """pairing_check_batch on bn254: checks[j] is a list of (bn254.G1.Point, bn254.G2.Point) pairs, True iff the

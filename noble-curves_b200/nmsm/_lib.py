@@ -44,6 +44,7 @@ EXPORTS = [
     "nmsm_secp256k1_recover_batch", "nmsm_secp256k1_ecrecover_batch",
     "nmsm_bls12_381_pairing_check_batch", "nmsm_bls12_381_verify_batch", "nmsm_bn254_pairing_check_batch",
     "nmsm_bls12_381_hash_to_g2_batch", "nmsm_bls12_381_verify_msg_batch", "nmsm_bls12_381_aggregate_verify_batch",
+    "nmsm_bls12_381_hash_to_g1_batch", "nmsm_bls12_381_short_verify_batch", "nmsm_bls12_381_short_verify_msg_batch",
 ]
 
 
@@ -190,6 +191,13 @@ def load() -> ctypes.CDLL:
         lib.nmsm_bls12_381_hash_to_g2_batch.restype = ctypes.c_int
         lib.nmsm_bls12_381_verify_msg_batch.argtypes = [u8p, u8p, u8p, u8p, ctypes.c_uint64, u8p, ctypes.c_uint64, u8p]
         lib.nmsm_bls12_381_verify_msg_batch.restype = ctypes.c_int
+        lib.nmsm_bls12_381_hash_to_g1_batch.argtypes = [u8p, u8p, ctypes.c_uint64, u8p, ctypes.c_uint64, u8p]
+        lib.nmsm_bls12_381_hash_to_g1_batch.restype = ctypes.c_int
+        lib.nmsm_bls12_381_short_verify_batch.argtypes = [u8p, u8p, u8p, ctypes.c_uint64, u8p]
+        lib.nmsm_bls12_381_short_verify_batch.restype = ctypes.c_int
+        lib.nmsm_bls12_381_short_verify_msg_batch.argtypes = [u8p, u8p, u8p, u8p, ctypes.c_uint64, u8p, ctypes.c_uint64,
+                                                              u8p]
+        lib.nmsm_bls12_381_short_verify_msg_batch.restype = ctypes.c_int
         lib.nmsm_bls12_381_aggregate_verify_batch.argtypes = [u8p, u8p, ctypes.c_uint64, u8p, u8p, u8p, u8p, u8p,
                                                               ctypes.c_uint64, u8p]
         lib.nmsm_bls12_381_aggregate_verify_batch.restype = ctypes.c_int
