@@ -24,6 +24,7 @@
  *   nmsm_ed25519_verify_each <- ed25519.verify over a batch, one verdict per signature (ZIP-215 or strict)
  *   nmsm_secp256k1_verify_batch <- secp256k1.verify over a batch, one verdict per signature (weierstrass.ts ecdsa().verify)
  *   nmsm_p256_verify_batch <- p256.verify over a batch, one verdict per signature (nist.ts; also EIP-7951 P256VERIFY)
+ *   nmsm_p384_verify_batch <- p384.verify over a batch, one verdict per signature (nist.ts)
  *   nmsm_secp256k1_schnorr_verify_batch <- schnorr.verify over a batch, one verdict per signature (secp256k1.ts, BIP340)
  *   nmsm_secp256k1_recover_batch <- secp256k1.recoverPublicKey over a batch (weierstrass.ts Signature.recoverPublicKey)
  *   nmsm_secp256k1_ecrecover_batch <- Ethereum's ecrecover precompile (0x01) over a batch
@@ -267,6 +268,19 @@ int nmsm_secp256k1_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, con
  * (17 x 2^15 points, 36 MB), kept until nmsm_shutdown.  With profiling on, nmsm_last_timing reports
  * k_p256_ecdsa_prepare in slot 0, k_p256_ecdsa_check in slot 1 and both in NMSM_T_TOTAL. */
 int nmsm_p256_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint64_t* pk_off, const uint8_t* msgs,
+                           const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
+
+/* P-384 (secp384r1) ECDSA batch verification: out_ok[i] = p384.verify(sig_i, msg_i, pk_i, { prehash, lowS }) with
+ * format 'compact' (noble-curves nist.ts / weierstrass.ts ecdsa().verify), one independent verdict per signature.
+ * Arguments, rules, errors and flags as nmsm_p256_verify_batch, on P-384 (y^2 = x^3 - 3x + b, SEC 2 §2.5.1): sigs are
+ * n x 96 B r || s, big-endian; keys are 49-byte SEC1 compressed or 97-byte uncompressed P-384 points (any other length
+ * is a 0 verdict).  NMSM_ECDSA_PREHASH hashes the message with SHA-384; h is the big-endian integer of the first
+ * min(len, 48) bytes of the (hashed or raw) message, reduced mod n.  noble's p384 defaults are { prehash: true,
+ * lowS: false }, i.e. flags = NMSM_ECDSA_PREHASH, which is also what OpenSSL checks.  The first call after nmsm_init
+ * builds the fixed-point table of the P-384 G (25 x 2^15 points of 96 B, 79 MB), kept until nmsm_shutdown.  With
+ * profiling on, nmsm_last_timing reports k_p384_ecdsa_prepare in slot 0, k_p384_ecdsa_check in slot 1 and both in
+ * NMSM_T_TOTAL. */
+int nmsm_p384_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint64_t* pk_off, const uint8_t* msgs,
                            const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
 
 /* secp256k1 BIP340 Schnorr batch verification (next-row f6): out_ok[i] = schnorr.verify(sig_i, msg_i, pk_i)

@@ -423,6 +423,8 @@ void nmsm_shutdown(void) {
   C.secp256k1_g_table = nullptr;
   cudaFree(C.p256_g_table);
   C.p256_g_table = nullptr;
+  cudaFree(C.p384_g_table);
+  C.p384_g_table = nullptr;
   cudaFree(C.ed25519_b_table);
   C.ed25519_b_table = nullptr;
   for (Buf* b : {&C.ntt_data, &C.ntt_work, &C.ntt_tmp, &C.ntt_roots, &C.ntt_aux}) b->release();
@@ -804,6 +806,20 @@ int nmsm_p256_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const ui
   if (!sigs || !pk_off || !msg_off || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
   if ((pk_off[n] && !pubkeys) || (msg_off[n] && !msgs)) return fail(NMSM_ERR_ARG, "null pointer");
   return p256_verify_batch_impl(sigs, pubkeys, pk_off, msgs, msg_off, n, flags, out_ok);
+}
+
+int nmsm_p384_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint64_t* pk_off, const uint8_t* msgs,
+                           const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (flags & ~(NMSM_ECDSA_PREHASH | NMSM_ECDSA_LOW_S)) return fail(NMSM_ERR_ARG, "nmsm_p384_verify_batch: unknown flag");
+  if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 31)) return fail(NMSM_ERR_ARG, "n must be < 2^31");  // before pk_off[n] / msg_off[n] are read
+  if (!sigs || !pk_off || !msg_off || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
+  if ((pk_off[n] && !pubkeys) || (msg_off[n] && !msgs)) return fail(NMSM_ERR_ARG, "null pointer");
+  return p384_verify_batch_impl(sigs, pubkeys, pk_off, msgs, msg_off, n, flags, out_ok);
 }
 
 int nmsm_secp256k1_schnorr_verify_batch(const uint8_t* sigs, const uint8_t* pubkeys, const uint8_t* msgs,

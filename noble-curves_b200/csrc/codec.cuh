@@ -1,7 +1,7 @@
 // Wire-format decoding on the GPU (SURVEY §8 row f2): bytes -> canonical affine (x, y) in the C-ABI packing,
 // so callers can hand the encodings the reference's `fromBytes` consumes instead of bigints.
 //   secp256k1  SEC1 compressed, 33 B      /root/reference/src/abstract/weierstrass.ts:565-588 (pointFromBytes)
-//              (the same decoder serves P-256 ECDSA keys, ecdsa_verify.cuh)
+//              (the same decoder serves P-256 and, 49 B, P-384 ECDSA keys, ecdsa_verify.cuh)
 //   BLS12-381 G1  Zcash-flag compressed, 48 B   src/bls12-381.ts:377-468 (coder.decode, parseMask/validateMask)
 //   BLS12-381 G2  Zcash-flag compressed, 96 B   same coder over Fp2 (c1 || c0, bls12-381.ts:354-367,488-491), Fp2 sqrt tower.ts:476-498
 //   ed25519    RFC 8032 / ZIP-215, 32 B   src/abstract/edwards.ts:405-436  (ed25519_verify.cuh ed_decompress)
@@ -48,16 +48,17 @@ NMSM_HD void words_from_be_bytes(uint32_t* w, const uint8_t* b) {  // big-endian
   }
 }
 
-// SEC1 compressed, 33 B: 02/03 || x, y = sqrt(x^3 + a x + b) with the prefix's parity, for a 256-bit prime field with
-// p = 3 (mod 4) (secp256k1, P-256).  status: 0 = invalid encoding, 1 = affine point written, 2 = point at infinity
-// ((0,0) written)
+// SEC1 compressed, 1 + 4 LIMBS bytes: 02/03 || x, y = sqrt(x^3 + a x + b) with the prefix's parity, for a prime field
+// with p = 3 (mod 4) (secp256k1 and P-256: 33 B; P-384: 49 B).  status: 0 = invalid encoding, 1 = affine point written,
+// 2 = point at infinity ((0,0) written)
 template <class Cv>
 NMSM_HD int sec1_decode_compressed(const uint8_t* enc, uint32_t* out_xy) {
   using F = typename Cv::G::Field;
+  constexpr int L = F::LIMBS;
   const uint8_t head = enc[0];
   if (head != 0x02 && head != 0x03) return 0;
-  uint32_t xw[8];
-  words_from_be_bytes<32>(xw, enc + 1);
+  uint32_t xw[L];
+  words_from_be_bytes<4 * L>(xw, enc + 1);
   if (!F::canonical_in_range(xw)) return 0;  // Fp.fromBytes rejects x >= p
   const F x = F::from_canonical(xw);
   F rhs;
@@ -71,15 +72,15 @@ NMSM_HD int sec1_decode_compressed(const uint8_t* enc, uint32_t* out_xy) {
   bool ok;
   F y = fp_sqrt_3mod4(rhs, ok);
   if (!ok) return 0;
-  uint32_t yw[8];
+  uint32_t yw[L];
   y.to_canonical(yw);
   if (((yw[0] & 1u) != 0) != ((head & 1u) != 0)) {
     y = -y;
     y.to_canonical(yw);
   }
-  for (int k = 0; k < 8; k++) {
+  for (int k = 0; k < L; k++) {
     out_xy[k] = xw[k];
-    out_xy[8 + k] = yw[k];
+    out_xy[L + k] = yw[k];
   }
   return 1;
 }

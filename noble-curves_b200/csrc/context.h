@@ -102,6 +102,7 @@ struct Context {
   uint32_t* secp256k1_g_table = nullptr;  // fixed-point table of the secp256k1 generator, built by the first verify
   uint32_t* ed25519_b_table = nullptr;    // fixed-point table of the ed25519 base point, built by the first verify_each
   uint32_t* p256_g_table = nullptr;       // fixed-point table of the P-256 generator, built by the first P-256 verify
+  uint32_t* p384_g_table = nullptr;       // fixed-point table of the P-384 generator, built by the first P-384 verify
   Buf ntt_data, ntt_work, ntt_tmp, ntt_roots, ntt_aux;  // NTT staging / work / output / root table (ntt.cu)
   int ntt_key_field = -1, ntt_key_bits = -1;            // which root table ntt_roots holds
   uint64_t ntt_key_gen = 0;
@@ -232,6 +233,8 @@ int ed25519_verify_each_impl(const uint8_t* sigs, const uint8_t* pks, const uint
 int secp256k1_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off, const uint8_t* msgs,
                                 const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
 int p256_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off, const uint8_t* msgs,
+                           const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
+int p384_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off, const uint8_t* msgs,
                            const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok);
 int secp256k1_schnorr_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs,
                                         const uint64_t* msg_off, uint64_t n, uint8_t* out_ok);

@@ -4,7 +4,7 @@
 // coordinates (weierstrass.ts:793-880 RCB, edwards.ts:505-545 hwcd).  Results are only defined up
 // to the projective representative, so parity is on canonical affine (x, y) (test/point.test.ts:36-44).
 // Here:
-//   * short Weierstrass a = 0 (secp256k1, bn254 G1/G2, BLS12-381 G1/G2) and a = -3 (P-256): XYZZ accumulators
+//   * short Weierstrass a = 0 (secp256k1, bn254 G1/G2, BLS12-381 G1/G2) and a = -3 (P-256, P-384): XYZZ accumulators
 //     (x = X/ZZ, y = Y/ZZZ, ZZ^3 = ZZZ^2; identity <=> ZZ == 0) with affine mixed addition
 //     madd-2008-s (8M+2S), add-2008-s (12M+2S), dbl-2008-s-1 (6M+3S for a=0; 7M+2S for a=-3), mdbl-2008-s-1.
 //     The incomplete formulas are completed by explicit branches for P+P, P+(-P), O+P, P+O — all
@@ -546,6 +546,17 @@ struct CurveP256 {
   using Fn = Fn_p256;
   static constexpr bool COFACTOR_ONE = true;
   static constexpr int ID = 8;
+};
+// NIST P-384 (secp384r1), a = -3 at 12 limbs: ECDSA verification only (inst_p384.cu), as P-256.  Scalars are 12 words
+// ((Fn::BITS + 31) / 32), the fixed-point table of G has 25 levels.  ID 9 is reserved for P-384; no curve-id entry point
+// of the C ABI accepts it.
+struct CurveP384 {
+  static constexpr bool GLV = false;
+  static constexpr int GLV_KIND = 0;
+  using G = SwXyzz<Fp<FpP384>, -3>;
+  using Fn = Fn_p384;
+  static constexpr bool COFACTOR_ONE = true;
+  static constexpr int ID = 9;
 };
 
 }  // namespace nmsm

@@ -1,42 +1,30 @@
-// ECDSA batch verification for secp256k1 (SURVEY §8 row f5) and P-256: one independent verdict per signature.
+// ECDSA batch verification for secp256k1 (SURVEY §8 row f5), P-256 and P-384: one independent verdict per signature.
 //
 // The reference verifies one signature at a time: weierstrass.ts `ecdsa().verify` (noble-curves v2), with
-// format 'compact' and the options { prehash, lowS } (both default true for secp256k1; p256 defaults to lowS false):
-//   sig = r || s (64 B, big-endian); inside the reference's try (any failure = false):
-//   1 <= r, s < n;  P = Point.fromBytes(publicKey)  (33 B 02/03 + sqrt, or 65 B 04 + curve equation);
-//   lowS && s > n/2 -> false;  h = bits2int_modN(prehash ? sha256(msg) : msg)  (bits2int: > 8192 bytes throws);
+// format 'compact' and the options { prehash, lowS } (both default true for secp256k1; p256 and p384 default to lowS
+// false).  For a curve with W-word field elements and scalars (W = 8, or 12 for P-384):
+//   sig = r || s (8W B, big-endian); inside the reference's try (any failure = false):
+//   1 <= r, s < n;  P = Point.fromBytes(publicKey)  (1 + 4W B 02/03 + sqrt, or 1 + 8W B 04 + curve equation);
+//   lowS && s > n/2 -> false;  h = bits2int_modN(prehash ? hash(msg) : msg)  (SHA-256, or SHA-384 for P-384;
+//   bits2int takes the first min(len, 4W) bytes, and throws above 8192 bytes);
 //   w = s^-1,  u1 = h w,  u2 = r w  (mod n);  R = u1 G + u2 P;  R == O -> false;  accept iff R.x mod n == r.
 // ECDSA has no batch equation (R's y is not in the signature), so the batch is data-parallel: per signature
-//   ecdsa_prepare_body  parse + range checks, lowS, key decode, SHA-256, bits2int mod n
+//   ecdsa_prepare_body  parse + range checks, lowS, key decode, prehash, bits2int mod n
 //   (kernel)            s^-1 through one warp-shared inversion per 32 signatures (msm.cuh warp_batch_inverse)
 //   ecdsa_store         u1, u2
 //   ecdsa_check_body    u1 G from the fixed-point table of G (table_mul_body), u2 Q (scalar_mul_acc: GLV on
-//                       secp256k1, plain windows on P-256), complete addition, and the x comparison in XYZZ
-//                       coordinates without an inversion.
-// The two halves run as two kernels (inst_secp256k1.cu, inst_p256.cu) so the SHA-256 / square-root state stays out of
-// the scalar multiplication's registers.  Bodies are host/device so tests/hostemu can run them.  They are templates on
-// the curve policy (CurveSecp256k1 by default, or CurveP256); what differs per curve is the group, the scalar modulus
-// n (EcdsaScalar) and the SEC1 key decoders.
+//                       secp256k1, plain windows on P-256 and P-384), complete addition, and the x comparison in
+//                       XYZZ coordinates without an inversion.
+// The two halves run as two kernels (inst_secp256k1.cu, inst_p256.cu, inst_p384.cu) so the hash / square-root state
+// stays out of the scalar multiplication's registers.  Bodies are host/device so tests/hostemu can run them.  They are
+// templates on the curve policy (CurveSecp256k1 by default, CurveP256 or CurveP384); what differs per curve is the
+// group and its width, the scalar modulus n and the prehash (EcdsaScalar) and the SEC1 key decoders.
 #pragma once
 #include "codec.cuh"
 #include "validate.cuh"
 
 namespace nmsm {
 
-// the scalar modulus n of each ECDSA curve (s^-1, u1, u2 mod n)
-template <class Cv>
-struct EcdsaScalar;
-template <>
-struct EcdsaScalar<CurveSecp256k1> {
-  using Mod = FnSecp256k1Mod;
-};
-template <>
-struct EcdsaScalar<CurveP256> {
-  using Mod = FnP256Mod;
-};
-template <class Cv>
-using EcdsaS = Fp<typename EcdsaScalar<Cv>::Mod>;
-using EcS = EcdsaS<CurveSecp256k1>;
 static constexpr int ECDSA_PREHASH = 1;  // include/nmsm.h NMSM_ECDSA_PREHASH
 static constexpr int ECDSA_LOW_S = 2;    // include/nmsm.h NMSM_ECDSA_LOW_S
 static constexpr uint64_t ECDSA_MAX_RAW_MSG = 8192;  // bits2int: "input is too large" above this many bytes
@@ -108,86 +96,127 @@ NMSM_HD void sha256(const uint8_t* msg, uint64_t len, uint8_t* out) {
   sha256_finish(st, 0, len, [&](uint64_t j) -> uint32_t { return msg[j]; }, out);
 }
 
-// SEC1 uncompressed, 65 B: 04 || x || y, x < p, y < p, on the curve (weierstrass.ts pointFromBytes, `isValidXY`).
-// (0, 0) is rejected although point_on_curve accepts it as the identity encoding: b != 0 on both curves.
-// status as sec1_decode_compressed: 0 = invalid, 1 = affine point written (canonical x, y words).
+// The per-curve ECDSA policy: the scalar modulus n (s^-1, u1, u2 mod n) and the prehash with its digest length
+template <class Cv>
+struct EcdsaScalar;
+template <>
+struct EcdsaScalar<CurveSecp256k1> {
+  using Mod = FnSecp256k1Mod;
+  static constexpr int DIGEST_BYTES = 32;
+  NMSM_HD static void prehash(const uint8_t* m, uint64_t len, uint8_t* out) { sha256(m, len, out); }
+};
+template <>
+struct EcdsaScalar<CurveP256> {
+  using Mod = FnP256Mod;
+  static constexpr int DIGEST_BYTES = 32;
+  NMSM_HD static void prehash(const uint8_t* m, uint64_t len, uint8_t* out) { sha256(m, len, out); }
+};
+template <>
+struct EcdsaScalar<CurveP384> {
+  using Mod = FnP384Mod;
+  static constexpr int DIGEST_BYTES = 48;
+  NMSM_HD static void prehash(const uint8_t* m, uint64_t len, uint8_t* out) { sha384(m, len, out); }
+};
+template <class Cv>
+using EcdsaS = Fp<typename EcdsaScalar<Cv>::Mod>;
+using EcS = EcdsaS<CurveSecp256k1>;
+// words of the curve's scalars (r, s, h, u1, u2) and of its field elements (the key's x, y).  Equal on every ECDSA curve
+// here (n and p have the same bit length), which lets r be compared with R.x in Fp.
+template <class Cv>
+NMSM_HD constexpr int ecdsa_sw() { return EcdsaS<Cv>::LIMBS; }
+template <class Cv>
+NMSM_HD constexpr int ecdsa_fw() { return Cv::G::Field::LIMBS; }
+
+// SEC1 uncompressed, 1 + 8 LIMBS bytes (65 B; 97 B on P-384): 04 || x || y, x < p, y < p, on the curve
+// (weierstrass.ts pointFromBytes, `isValidXY`).  (0, 0) is rejected although point_on_curve accepts it as the identity
+// encoding: b != 0 on every ECDSA curve.  status as sec1_decode_compressed: 0 = invalid, 1 = affine point written
+// (canonical x, y words).
 template <class Cv>
 NMSM_HD int sec1_decode_uncompressed(const uint8_t* enc, uint32_t* out_xy) {
+  constexpr int L = Cv::G::Field::LIMBS;
   if (enc[0] != 0x04) return 0;
-  uint32_t xy[16];
-  words_from_be_bytes<32>(xy, enc + 1);
-  words_from_be_bytes<32>(xy + 8, enc + 33);
+  uint32_t xy[2 * L];
+  words_from_be_bytes<4 * L>(xy, enc + 1);
+  words_from_be_bytes<4 * L>(xy + L, enc + 1 + 4 * L);
   uint32_t any = 0;
-  for (int k = 0; k < 16; k++) any |= xy[k];
+  for (int k = 0; k < 2 * L; k++) any |= xy[k];
   if (any == 0 || !point_on_curve<Cv>(xy)) return 0;
-  for (int k = 0; k < 16; k++) out_xy[k] = xy[k];
+  for (int k = 0; k < 2 * L; k++) out_xy[k] = xy[k];
   return 1;
 }
 NMSM_HD int sec1_decode_secp256k1_uncompressed(const uint8_t* enc, uint32_t* out_xy) {
   return sec1_decode_uncompressed<CurveSecp256k1>(enc, out_xy);
 }
 
-NMSM_HD bool words8_nonzero(const uint32_t* a) {
+template <int W>
+NMSM_HD bool words_nonzero(const uint32_t* a) {
   uint32_t t = 0;
-  for (int k = 0; k < 8; k++) t |= a[k];
+  for (int k = 0; k < W; k++) t |= a[k];
   return t != 0;
 }
+NMSM_HD bool words8_nonzero(const uint32_t* a) { return words_nonzero<8>(a); }
 // a > (n >> 1): the high-S test (Signature.hasHighS)
 template <class Cv = CurveSecp256k1>
 NMSM_HD bool ecdsa_high_s(const uint32_t* s) {
   using Mod = typename EcdsaScalar<Cv>::Mod;
-  for (int k = 7; k >= 0; k--) {
-    const uint32_t half = (Mod::P(k) >> 1) | (k < 7 ? Mod::P(k + 1) << 31 : 0u);
+  constexpr int SW = ecdsa_sw<Cv>();
+  for (int k = SW - 1; k >= 0; k--) {
+    const uint32_t half = (Mod::P(k) >> 1) | (k < SW - 1 ? Mod::P(k + 1) << 31 : 0u);
     if (s[k] != half) return s[k] > half;
   }
   return false;
 }
 
-// h = bits2int_modN(prehash ? sha256(m) : m) for the message m[0..mlen): the big-endian integer of the first
-// min(len, 32) bytes, reduced mod n.  False for a raw message over ECDSA_MAX_RAW_MSG bytes (bits2int throws).
+// h = bits2int_modN(prehash ? hash(m) : m) for the message m[0..mlen): the big-endian integer of the first
+// min(len, 4 SW) bytes (32, or 48 on P-384: n has 32 SW bits), reduced mod n.  False for a raw message over
+// ECDSA_MAX_RAW_MSG bytes (bits2int throws).
 template <class Cv = CurveSecp256k1>
 NMSM_HD bool ecdsa_msg_hash(const uint8_t* m, uint64_t mlen, int flags, uint32_t* h) {
-  using Mod = typename EcdsaScalar<Cv>::Mod;
-  uint8_t digest[32];
+  using Pol = EcdsaScalar<Cv>;
+  using Mod = typename Pol::Mod;
+  constexpr int SW = ecdsa_sw<Cv>(), NB = 4 * SW;
+  uint8_t digest[Pol::DIGEST_BYTES];
   if (flags & ECDSA_PREHASH) {
-    sha256(m, mlen, digest);
+    Pol::prehash(m, mlen, digest);
     m = digest;
-    mlen = 32;
+    mlen = Pol::DIGEST_BYTES;
   } else if (mlen > ECDSA_MAX_RAW_MSG) {
     return false;
   }
-  const int take = mlen < 32 ? (int)mlen : 32;
-  for (int k = 0; k < 8; k++) h[k] = 0;
+  const int take = mlen < NB ? (int)mlen : NB;
+  for (int k = 0; k < SW; k++) h[k] = 0;
   for (int j = 0; j < take; j++) {
     const int bit = 8 * (take - 1 - j);
     h[bit >> 5] |= (uint32_t)m[j] << (bit & 31);
   }
-  if (!EcdsaS<Cv>::canonical_in_range(h)) {  // h < 2^256 < 2n: one subtraction reduces it
+  if (!EcdsaS<Cv>::canonical_in_range(h)) {  // h < 2^(32 SW) < 2n: one subtraction reduces it
     h[0] = sub_cc(h[0], Mod::P(0));
-    for (int k = 1; k < 8; k++) h[k] = subc_cc(h[k], Mod::P(k));
+    for (int k = 1; k < SW; k++) h[k] = subc_cc(h[k], Mod::P(k));
   }
   return true;
 }
 
-// Signature i: r, s, the public key Q (canonical affine words) and h = bits2int_modN(m).  False = the reference's
+// Signature i: r, s, h (SW words each), the public key Q (2 FW canonical affine words) and h = bits2int_modN(m).  False = the reference's
 // verify returns false before any scalar multiplication; the outputs are then unspecified.
 template <class Cv = CurveSecp256k1>
 NMSM_HD bool ecdsa_prepare_body(uint32_t i, const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off,
                                 const uint8_t* msgs, const uint64_t* msg_off, int flags, uint32_t* q_xy, uint32_t* r,
                                 uint32_t* s, uint32_t* h) {
-  const uint8_t* sig = sigs + (size_t)i * 64;
-  words_from_be_bytes<32>(r, sig);
-  words_from_be_bytes<32>(s, sig + 32);
+  constexpr int SW = ecdsa_sw<Cv>(), FW = ecdsa_fw<Cv>();
+  const uint8_t* sig = sigs + (size_t)i * (8 * SW);
+  words_from_be_bytes<4 * SW>(r, sig);
+  words_from_be_bytes<4 * SW>(s, sig + 4 * SW);
   // Signature.fromBytes: 1 <= r < n, 1 <= s < n;  then lowS
   using S = EcdsaS<Cv>;
-  if (!words8_nonzero(r) || !S::canonical_in_range(r) || !words8_nonzero(s) || !S::canonical_in_range(s)) return false;
+  if (!words_nonzero<SW>(r) || !S::canonical_in_range(r) || !words_nonzero<SW>(s) || !S::canonical_in_range(s))
+    return false;
   if ((flags & ECDSA_LOW_S) && ecdsa_high_s<Cv>(s)) return false;
   // Point.fromBytes
   const uint8_t* pk = pks + pk_off[i];
   const uint64_t pk_len = pk_off[i + 1] - pk_off[i];
-  if (pk_len == 33) {
+  if (pk_len == 1 + 4 * FW) {
     if (sec1_decode_compressed<Cv>(pk, q_xy) != 1) return false;
-  } else if (pk_len == 65) {
+  } else if (pk_len == 1 + 8 * FW) {
     if (sec1_decode_uncompressed<Cv>(pk, q_xy) != 1) return false;
   } else {
     return false;
@@ -201,24 +230,27 @@ template <class Cv = CurveSecp256k1>
 NMSM_HD void ecdsa_store(uint32_t i, bool ok, const uint32_t* q_xy, const uint32_t* r, const uint32_t* h,
                          const EcdsaS<Cv>& w, uint32_t* qs, uint32_t* u1s, uint32_t* u2s, uint32_t* rs, uint8_t* ok_out) {
   using S = EcdsaS<Cv>;
+  constexpr int SW = ecdsa_sw<Cv>(), FW = ecdsa_fw<Cv>();
   ok_out[i] = ok ? 1 : 0;
   if (!ok) return;
-  uint32_t u1[8], u2[8];
+  uint32_t u1[SW], u2[SW];
   (S::from_canonical(h) * w).to_canonical(u1);
   (S::from_canonical(r) * w).to_canonical(u2);
-  store_words<16>(qs + (size_t)i * 16, q_xy);
-  store_words<8>(u1s + (size_t)i * 8, u1);
-  store_words<8>(u2s + (size_t)i * 8, u2);
-  store_words<8>(rs + (size_t)i * 8, r);
+  store_words<2 * FW>(qs + (size_t)i * (2 * FW), q_xy);
+  store_words<SW>(u1s + (size_t)i * SW, u1);
+  store_words<SW>(u2s + (size_t)i * SW, u2);
+  store_words<SW>(rs + (size_t)i * SW, r);
 }
 
-// serial statement of k_ecdsa_prepare / k_p256_ecdsa_prepare (one inversion per signature instead of one per warp)
+// serial statement of k_ecdsa_prepare / k_p256_ecdsa_prepare / k_p384_ecdsa_prepare (one inversion per signature
+// instead of one per warp)
 template <class Cv = CurveSecp256k1>
 NMSM_HD void ecdsa_prepare_serial(uint32_t n, const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off,
                                   const uint8_t* msgs, const uint64_t* msg_off, int flags, uint32_t* qs, uint32_t* u1s,
                                   uint32_t* u2s, uint32_t* rs, uint8_t* ok_out) {
+  constexpr int SW = ecdsa_sw<Cv>(), FW = ecdsa_fw<Cv>();
   for (uint32_t i = 0; i < n; i++) {
-    uint32_t q[16], r[8], s[8], h[8];
+    uint32_t q[2 * FW], r[SW], s[SW], h[SW];
     const bool ok = ecdsa_prepare_body<Cv>(i, sigs, pks, pk_off, msgs, msg_off, flags, q, r, s, h);
     using S = EcdsaS<Cv>;
     ecdsa_store<Cv>(i, ok, q, r, h, ok ? inv(S::from_canonical(s)) : S::one(), qs, u1s, u2s, rs, ok_out);
@@ -226,16 +258,19 @@ NMSM_HD void ecdsa_prepare_serial(uint32_t n, const uint8_t* sigs, const uint8_t
 }
 
 // R.x mod n == r for R = acc (XYZZ, x = X / ZZ), without an inversion: X == r ZZ, or, when r + n < p (R.x >= n is
-// possible because p - n < 2^128 on both curves), X == (r + n) ZZ.  R = O (ZZ = 0) is false.
+// possible because n < p < 2n on every curve here: p - n < 2^128 on the 256-bit curves, < 2^190 on P-384),
+// X == (r + n) ZZ.  R = O (ZZ = 0) is false.
 template <class Cv = CurveSecp256k1>
 NMSM_HD bool ecdsa_x_matches(const typename Cv::G::Acc& acc, const uint32_t* r) {
   using F = typename Cv::G::Field;
   using Mod = typename EcdsaScalar<Cv>::Mod;
+  constexpr int W = ecdsa_fw<Cv>();
+  static_assert(ecdsa_sw<Cv>() == W, "ecdsa_x_matches: r and R.x must have the same width");
   if (Cv::G::is_identity(acc)) return false;
   if (acc.X == F::from_canonical(r) * acc.ZZ) return true;  // r < n < p
-  uint32_t rn[8];
+  uint32_t rn[W];
   rn[0] = add_cc(r[0], Mod::P(0));
-  for (int k = 1; k < 8; k++) rn[k] = addc_cc(r[k], Mod::P(k));
+  for (int k = 1; k < W; k++) rn[k] = addc_cc(r[k], Mod::P(k));
   const uint32_t carry = addc(0, 0);
   if (carry || !F::canonical_in_range(rn)) return false;
   return acc.X == F::from_canonical(rn) * acc.ZZ;
@@ -243,18 +278,20 @@ NMSM_HD bool ecdsa_x_matches(const typename Cv::G::Acc& acc, const uint32_t* r) 
 
 // Signature i after ecdsa_store: R = u1 G + u2 Q, out_ok[i] = verdict.  tbl: the fixed-point table of G
 // (table_mul_body layout, BITS-bit digits; BITS is a parameter only so that tests/hostemu can use a small table).
-// u2 Q: GLV windows on secp256k1, plain 4-bit windows on P-256 (scalar_mul_acc).
+// u2 Q: GLV windows on secp256k1, plain 4-bit windows on P-256 and P-384 (scalar_mul_acc).
 template <int BITS = PT_BITS, class Cv = CurveSecp256k1>
 NMSM_HD void ecdsa_check_body(uint32_t i, const uint32_t* tbl, const uint32_t* qs, const uint32_t* u1s,
                               const uint32_t* u2s, const uint32_t* rs, uint8_t* out_ok, unsigned int* err) {
   using G = typename Cv::G;
+  constexpr int SW = ecdsa_sw<Cv>(), FW = ecdsa_fw<Cv>();
+  static_assert(scalar_words<typename Cv::Fn>() == SW, "ecdsa_check_body: table_mul_body reads SW-word scalars");
   if (!out_ok[i]) return;
   typename G::Acc acc;
   table_mul_body<Cv, BITS>(i, tbl, u1s, 1, acc, err);  // u1 < n always; u1 = 0 (h = 0 mod n) gives O
-  uint32_t q[16], u2[8], r[8];
-  load_words<16>(q, qs + (size_t)i * 16);
-  load_words<8>(u2, u2s + (size_t)i * 8);
-  load_words<8>(r, rs + (size_t)i * 8);
+  uint32_t q[2 * FW], u2[SW], r[SW];
+  load_words<2 * FW>(q, qs + (size_t)i * (2 * FW));
+  load_words<SW>(u2, u2s + (size_t)i * SW);
+  load_words<SW>(r, rs + (size_t)i * SW);
   nl_add<G>(acc, scalar_mul_acc<Cv>(G::prepare(q), u2));  // complete: doubles when u1 G == u2 Q
   out_ok[i] = ecdsa_x_matches<Cv>(acc, r) ? 1 : 0;
 }

@@ -132,6 +132,28 @@ NMSM_HD uint64_t sha512_k(int i) {
 }
 NMSM_HD uint64_t rotr64(uint64_t x, int n) { return (x >> n) | (x << (64 - n)); }
 
+// One SHA-512 compression (FIPS 180-4 §6.4.2): st <- st + the 80 rounds over the block w[16] (big-endian 64-bit words;
+// w is overwritten).  SHA-512 and SHA-384 share it.
+NMSM_HD void sha512_compress(uint64_t* st, uint64_t* w) {
+  uint64_t a = st[0], bb = st[1], c = st[2], d = st[3], e = st[4], f = st[5], g = st[6], h = st[7];
+  for (int i = 0; i < 80; i++) {
+    if (i >= 16) {
+      const uint64_t w15 = w[(i - 15) & 15], w2 = w[(i - 2) & 15];
+      const uint64_t s0 = rotr64(w15, 1) ^ rotr64(w15, 8) ^ (w15 >> 7);
+      const uint64_t s1 = rotr64(w2, 19) ^ rotr64(w2, 61) ^ (w2 >> 6);
+      w[i & 15] = w[i & 15] + s0 + w[(i - 7) & 15] + s1;
+    }
+    const uint64_t S1 = rotr64(e, 14) ^ rotr64(e, 18) ^ rotr64(e, 41);
+    const uint64_t ch = (e & f) ^ (~e & g);
+    const uint64_t t1 = h + S1 + ch + sha512_k(i) + w[i & 15];
+    const uint64_t S0 = rotr64(a, 28) ^ rotr64(a, 34) ^ rotr64(a, 39);
+    const uint64_t mj = (a & bb) ^ (a & c) ^ (bb & c);
+    const uint64_t t2 = S0 + mj;
+    h = g; g = f; f = e; e = d + t1; d = c; c = bb; bb = a; a = t1 + t2;
+  }
+  st[0] += a; st[1] += bb; st[2] += c; st[3] += d; st[4] += e; st[5] += f; st[6] += g; st[7] += h;
+}
+
 // SHA-512(R || A || M); digest as 64 bytes little-endian-interpretable words out[0..15] (u32, byte order of the digest)
 NMSM_HD void sha512_rAM(const uint8_t* r32, const uint8_t* a32, const uint8_t* msg, uint64_t mlen, uint8_t* digest) {
   uint64_t st[8] = {0x6a09e667f3bcc908ULL, 0xbb67ae8584caa73bULL, 0x3c6ef372fe94f82bULL, 0xa54ff53a5f1d36f1ULL,
@@ -154,26 +176,36 @@ NMSM_HD void sha512_rAM(const uint8_t* r32, const uint8_t* a32, const uint8_t* m
       for (int k = 0; k < 8; k++) x = (x << 8) | byte_at(b * 128 + 8 * i + k);
       w[i] = x;
     }
-    uint64_t a = st[0], bb = st[1], c = st[2], d = st[3], e = st[4], f = st[5], g = st[6], h = st[7];
-    for (int i = 0; i < 80; i++) {
-      if (i >= 16) {
-        const uint64_t w15 = w[(i - 15) & 15], w2 = w[(i - 2) & 15];
-        const uint64_t s0 = rotr64(w15, 1) ^ rotr64(w15, 8) ^ (w15 >> 7);
-        const uint64_t s1 = rotr64(w2, 19) ^ rotr64(w2, 61) ^ (w2 >> 6);
-        w[i & 15] = w[i & 15] + s0 + w[(i - 7) & 15] + s1;
-      }
-      const uint64_t S1 = rotr64(e, 14) ^ rotr64(e, 18) ^ rotr64(e, 41);
-      const uint64_t ch = (e & f) ^ (~e & g);
-      const uint64_t t1 = h + S1 + ch + sha512_k(i) + w[i & 15];
-      const uint64_t S0 = rotr64(a, 28) ^ rotr64(a, 34) ^ rotr64(a, 39);
-      const uint64_t mj = (a & bb) ^ (a & c) ^ (bb & c);
-      const uint64_t t2 = S0 + mj;
-      h = g; g = f; f = e; e = d + t1; d = c; c = bb; bb = a; a = t1 + t2;
-    }
-    st[0] += a; st[1] += bb; st[2] += c; st[3] += d; st[4] += e; st[5] += f; st[6] += g; st[7] += h;
+    sha512_compress(st, w);
   }
   for (int i = 0; i < 8; i++)
     for (int k = 0; k < 8; k++) digest[8 * i + k] = (uint8_t)(st[i] >> (56 - 8 * k));
+}
+
+// SHA-384(msg[0..len)) -> out[48], the digest's byte order: SHA-512's compression from the FIPS 180-4 §5.3.4 initial
+// value, truncated to the first six state words (the P-384 ECDSA prehash, ecdsa_verify.cuh)
+NMSM_HD void sha384(const uint8_t* msg, uint64_t len, uint8_t* out) {
+  uint64_t st[8] = {0xcbbb9d5dc1059ed8ULL, 0x629a292a367cd507ULL, 0x9159015a3070dd17ULL, 0x152fecd8f70e5939ULL,
+                    0x67332667ffc00b31ULL, 0x8eb44a8768581511ULL, 0xdb0c2e0d64f98fa7ULL, 0x47b5481dbefa4fa4ULL};
+  const uint64_t nblocks = (len + 1 + 16 + 127) / 128;
+  const uint64_t end = nblocks * 128;
+  auto byte_at = [&](uint64_t j) -> uint32_t {  // j-th byte of the padded message
+    if (j < len) return msg[j];
+    if (j == len) return 0x80u;
+    if (j >= end - 8) return (uint32_t)(((len * 8) >> (8 * (end - 1 - j))) & 0xff);  // 128-bit length, high half zero
+    return 0u;
+  };
+  for (uint64_t b = 0; b < nblocks; b++) {
+    uint64_t w[16];
+    for (int i = 0; i < 16; i++) {
+      uint64_t x = 0;
+      for (int k = 0; k < 8; k++) x = (x << 8) | byte_at(b * 128 + 8 * i + k);
+      w[i] = x;
+    }
+    sha512_compress(st, w);
+  }
+  for (int i = 0; i < 6; i++)
+    for (int k = 0; k < 8; k++) out[8 * i + k] = (uint8_t)(st[i] >> (56 - 8 * k));
 }
 
 NMSM_HD void words_from_le_bytes(uint32_t* w, const uint8_t* b, int nwords) {

@@ -413,11 +413,16 @@ NMSM_HD uint32_t scalar_bits(const uint32_t* s, int off, int c, int nwords = SCA
   return (uint32_t)v & ((1u << c) - 1u);
 }
 
+// words of a scalar below the order of Fn: 8 for every curve id of the MSM (SCALAR_WORDS, its input layout), 12 for
+// P-384, whose ECDSA bodies pass 12-word scalars to table_mul_body and scalar_mul_acc
+template <class Fn>
+NMSM_HD constexpr int scalar_words() { return (Fn::BITS + 31) / 32; }
+
 template <class Fn>
 NMSM_HD bool scalar_in_range(const uint32_t* s) {
   uint32_t t = sub_cc(s[0], Fn::ORDER(0));
 #pragma unroll
-  for (int k = 1; k < SCALAR_WORDS; k++) t = subc_cc(s[k], Fn::ORDER(k));
+  for (int k = 1; k < scalar_words<Fn>(); k++) t = subc_cc(s[k], Fn::ORDER(k));
   (void)t;
   return subc(0, 0) != 0;
 }
@@ -770,17 +775,18 @@ NMSM_HD void table_base_body(uint32_t i, const uint32_t* p_aff, uint32_t* level0
   store_words<G::AFF_WORDS>(level0 + (size_t)i * G::AFF_WORDS, reinterpret_cast<const uint32_t*>(&a));
 }
 
-// k * P from the table as an un-normalised accumulator.  Returns false (and records the index) for a scalar
+// k * P from the table as an un-normalised accumulator; scalars are scalar_words<Fn>() words each.  Returns false (and records the index) for a scalar
 // outside Point.multiply's range 1 <= k < n (allow_zero: multiplyUnsafe's 0 <= k < n).
 template <class Cv, int BITS = PT_BITS>
 NMSM_HD bool table_mul_body(uint32_t i, const uint32_t* tbl, const uint32_t* scalars, int allow_zero,
                             typename Cv::G::Acc& acc, unsigned int* err) {
   using G = typename Cv::G;
   constexpr uint32_t HALF = 1u << (BITS - 1);
-  uint32_t s[SCALAR_WORDS];
-  load_words<SCALAR_WORDS>(s, scalars + (size_t)i * SCALAR_WORDS);
+  constexpr int SW = scalar_words<typename Cv::Fn>();
+  uint32_t s[SW];
+  load_words<SW>(s, scalars + (size_t)i * SW);
   uint32_t nz = 0;
-  for (int k = 0; k < SCALAR_WORDS; k++) nz |= s[k];
+  for (int k = 0; k < SW; k++) nz |= s[k];
   acc = G::identity();
   if (!scalar_in_range<typename Cv::Fn>(s) || (!allow_zero && nz == 0)) {
     atomic_min_u32(&err[1], i);
@@ -789,7 +795,7 @@ NMSM_HD bool table_mul_body(uint32_t i, const uint32_t* tbl, const uint32_t* sca
   uint32_t carry = 0;
   constexpr int LEVELS = point_table_levels<Cv, BITS>();
   for (int w = 0; w < LEVELS; w++) {
-    uint32_t v = scalar_bits(s, w * BITS, BITS) + carry;
+    uint32_t v = scalar_bits(s, w * BITS, BITS, SW) + carry;
     carry = 0;
     bool neg = false;
     if (v > HALF) {
@@ -1401,7 +1407,7 @@ NMSM_HD int mul_window_digit(const uint32_t* m, int nwords, int w, uint32_t& car
   return (int)v;
 }
 
-// s * P as an un-normalised accumulator (the core of mul_body / torsion_body); s < n, 8 words
+// s * P as an un-normalised accumulator (the core of mul_body / torsion_body); s < n, scalar_words<Fn>() words
 // Ops: SerialOps (one thread per item) or msm.cuh QuadOps (one item per quad of lanes, k_mul_batch for small batches).
 template <class Cv, class Ops = SerialOps<typename Cv::G>>
 NMSM_HD typename Cv::G::Acc scalar_mul_acc(const typename Cv::G::Affine& P, const uint32_t* s) {
@@ -1455,7 +1461,7 @@ NMSM_HD typename Cv::G::Acc scalar_mul_acc(const typename Cv::G::Affine& P, cons
     constexpr int NW = (Cv::Fn::BITS + 1 + MUL_WBITS - 1) / MUL_WBITS;
     signed char dg[NW];
     uint32_t c = 0;
-    for (int w = 0; w < NW; w++) dg[w] = (signed char)mul_window_digit(s, SCALAR_WORDS, w, c);
+    for (int w = 0; w < NW; w++) dg[w] = (signed char)mul_window_digit(s, scalar_words<typename Cv::Fn>(), w, c);
     for (int w = NW - 1; w >= 0; w--) {
       if (w != NW - 1)
         for (int j = 0; j < MUL_WBITS; j++) Ops::dbl(acc);

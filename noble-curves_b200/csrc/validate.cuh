@@ -16,7 +16,7 @@ NMSM_HD F field_from_small(uint32_t v) {
 }
 
 // curve constant b of y^2 = x^3 + a x + b (secp256k1.ts:48-56, bn254.ts:80-90,207-223, bls12-381.ts:134-148,321-345;
-// P-256: SEC 2 §2.4.2)
+// P-256, P-384: SEC 2 §2.4.2, §2.5.1)
 template <class Cv>
 NMSM_HD typename Cv::G::Field curve_b() {
   using F = typename Cv::G::Field;
@@ -24,6 +24,11 @@ NMSM_HD typename Cv::G::Field curve_b() {
   else if constexpr (Cv::ID == 8) {
     F b;
     for (int k = 0; k < F::LIMBS; k++) b.v[k] = P256Consts::B_MONT(k);
+    return b;
+  }
+  else if constexpr (Cv::ID == 9) {
+    F b;
+    for (int k = 0; k < F::LIMBS; k++) b.v[k] = P384Consts::B_MONT(k);
     return b;
   }
   else if constexpr (Cv::ID == 2) return field_from_small<F>(3);

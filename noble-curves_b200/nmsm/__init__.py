@@ -939,7 +939,7 @@ def _pack_offsets(items) -> bytes:
     return struct.pack("<%dQ" % len(offs), *offs)
 
 
-def _check_ecdsa_args(signatures, messages, public_keys):
+def _check_ecdsa_args(signatures, messages, public_keys, sig_len: int = 64):
     n = len(signatures)
     if len(messages) != n or len(public_keys) != n:
         raise ValueError("signatures, messages and public keys must have equal length")
@@ -948,8 +948,8 @@ def _check_ecdsa_args(signatures, messages, public_keys):
             if not isinstance(x, (bytes, bytearray, memoryview)):
                 raise TypeError('"%s" expected Uint8Array, got type=%s' % (what, type(x).__name__))
     for s in signatures:
-        if len(s) != 64:
-            raise ValueError('"compact signature" expected Uint8Array of length 64, got length=%d' % len(s))
+        if len(s) != sig_len:
+            raise ValueError('"compact signature" expected Uint8Array of length %d, got length=%d' % (sig_len, len(s)))
 
 
 def ecdsa_verify_batch(signatures, messages, public_keys, prehash: bool = True, lowS: bool = True) -> List[bool]:
@@ -1083,6 +1083,53 @@ def p256verify_precompile_batch(inputs) -> List[bool]:
     res = p256_ecdsa_verify_batch_packed(sigs, keys.tobytes(), off(65), msgs, off(32), m, 0)
     out[idx] = np.frombuffer(res, np.uint8) == 1
     return out.tolist()
+
+
+def p384_ecdsa_verify_batch(signatures, messages, public_keys, prehash: bool = True, lowS: bool = False) -> List[bool]:
+    """Batch form of p384.verify(sig, msg, publicKey, {prehash, lowS}) with format 'compact' (noble-curves nist.ts,
+    weierstrass.ts ecdsa().verify): one verdict per signature.  Signatures are 96 bytes r || s, keys 49-byte compressed
+    or 97-byte uncompressed SEC1, and prehash hashes with SHA-384.  The defaults are noble's for p384 (lowS false, as
+    OpenSSL).  Raises as p256_ecdsa_verify_batch; everything else (r, s out of range, high s under lowS, an undecodable
+    key, a raw message over 8192 bytes, R = O) is a False verdict."""
+    _check_ecdsa_args(signatures, messages, public_keys, sig_len=96)
+    flags = (ECDSA_PREHASH if prehash else 0) | (ECDSA_LOW_S if lowS else 0)
+    out = p384_ecdsa_verify_batch_packed(b"".join(bytes(s) for s in signatures),
+                                         b"".join(bytes(p) for p in public_keys), _pack_offsets(public_keys),
+                                         b"".join(bytes(m) for m in messages), _pack_offsets(messages),
+                                         len(signatures), flags)
+    return [b == 1 for b in out]
+
+
+def p384_ecdsa_verify_batch_packed(sigs: bytes, pks: bytes, pk_off: bytes, msgs: bytes, msg_off: bytes, n: int,
+                                   flags: int = ECDSA_PREHASH) -> bytes:
+    """The C-ABI call itself (nmsm_p384_verify_batch) on caller-packed arrays: n*96 signature bytes, the concatenated
+    keys and messages with n+1 little-endian u64 offsets each.  Returns n verdict bytes (1 = valid)."""
+    if len(sigs) != 96 * n or len(pk_off) != 8 * (n + 1) or len(msg_off) != 8 * (n + 1):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    rc = lib.nmsm_p384_verify_batch(cp(sigs or b"\0"), cp(pks or b"\0"), cp(pk_off), cp(msgs or b"\0"), cp(msg_off), n,
+                                    flags, out)
+    try:
+        _lib.check(rc)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return out.raw[:n]
+
+
+def _p384_verify(signature, message, publicKey, prehash: bool = True, lowS: bool = False,
+                 format: str = "compact") -> bool:
+    """p384.verify for one signature (the batch entry point with n = 1)."""
+    if format != "compact":
+        raise NotImplementedError("signature format %r is not part of the accelerated path (compact only)" % (format,))
+    return p384_ecdsa_verify_batch([signature], [message], [publicKey], prehash=prehash, lowS=lowS)[0]
+
+
+# noble-curves' `p384` export (nist.ts; also `secp384r1`).  Verification only, as p256: not in CURVES.
+p384 = _NS(verify=_p384_verify)
+secp384r1 = p384
 
 
 def schnorr_verify_batch(signatures, messages, public_keys) -> List[bool]:

@@ -40,7 +40,7 @@ EXPORTS = [
     "nmsm_ed25519_verify_batch", "nmsm_ed25519_verify_each", "nmsm_msm_submit", "nmsm_msm_collect", "nmsm_points_decode", "nmsm_msm_submit_partial",
     "nmsm_points_decode_ex", "nmsm_points_on_curve", "nmsm_set_window_groups", "nmsm_accs_normalize",
     "nmsm_dist_unique_id", "nmsm_dist_init", "nmsm_dist_info", "nmsm_dist_exchange_mode", "nmsm_msm_sharded", "nmsm_msm_sharded_submit",
-    "nmsm_secp256k1_verify_batch", "nmsm_p256_verify_batch", "nmsm_secp256k1_schnorr_verify_batch",
+    "nmsm_secp256k1_verify_batch", "nmsm_p256_verify_batch", "nmsm_p384_verify_batch", "nmsm_secp256k1_schnorr_verify_batch",
     "nmsm_secp256k1_recover_batch", "nmsm_secp256k1_ecrecover_batch",
     "nmsm_bls12_381_pairing_check_batch", "nmsm_bls12_381_verify_batch", "nmsm_bn254_pairing_check_batch",
     "nmsm_bls12_381_hash_to_g2_batch", "nmsm_bls12_381_verify_msg_batch", "nmsm_bls12_381_aggregate_verify_batch",
@@ -175,6 +175,8 @@ def load() -> ctypes.CDLL:
         lib.nmsm_secp256k1_verify_batch.restype = ctypes.c_int
         lib.nmsm_p256_verify_batch.argtypes = [u8p, u8p, u8p, u8p, u8p, ctypes.c_uint64, ctypes.c_int, u8p]
         lib.nmsm_p256_verify_batch.restype = ctypes.c_int
+        lib.nmsm_p384_verify_batch.argtypes = [u8p, u8p, u8p, u8p, u8p, ctypes.c_uint64, ctypes.c_int, u8p]
+        lib.nmsm_p384_verify_batch.restype = ctypes.c_int
         lib.nmsm_secp256k1_schnorr_verify_batch.argtypes = [u8p, u8p, u8p, u8p, ctypes.c_uint64, u8p]
         lib.nmsm_secp256k1_schnorr_verify_batch.restype = ctypes.c_int
         lib.nmsm_secp256k1_recover_batch.argtypes = [u8p, u8p, u8p, ctypes.c_uint64, ctypes.c_int, u8p, u8p]
