@@ -35,6 +35,8 @@
  *   nmsm_bls12_381_hash_to_g1_batch <- bls12_381.G1.hashToCurve(msg, { DST }) over a batch (RFC 9380)
  *   nmsm_bls12_381_short_verify_batch / _msg_batch <- bls12_381.verifyShortSignature over a batch (key in G2,
  *                                                    signature in G1; messages hashed to G1 before or on the GPU)
+ *   nmsm_bls12_381_kzg_verify_proof_batch / _blob_batch <- EIP-4844 verify_kzg_proof (and the point-evaluation
+ *                                                    precompile 0x0A) / verify_blob_kzg_proof over a batch
  *   nmsm_ntt           <- FFT(rootsOfUnity(Fr, G), Fr).direct / .inverse   src/abstract/fft.ts:518-575
  *
  * Data formats (all little-endian, plain bytes, caller-owned):
@@ -447,6 +449,40 @@ int nmsm_bls12_381_short_verify_batch(const uint8_t* sigs48, const uint8_t* pks9
 int nmsm_bls12_381_short_verify_msg_batch(const uint8_t* sigs48, const uint8_t* pks96, const uint8_t* msgs,
                                           const uint64_t* msg_off, uint64_t n, const uint8_t* dst, uint64_t dst_len,
                                           uint8_t* out_ok);
+
+/* EIP-4844 KZG proof verification on BLS12-381 (next-row f15), one independent verdict per item, with the rules of the
+ * consensus specs (Deneb polynomial-commitments.md).  Field elements (z, y, blob elements) are 32-byte BIG-endian and
+ * must be < r = 0x73eda753...ffffffff00000001; points are 48-byte Zcash-flag compressed G1 encodings checked as
+ * validate_kzg_g1 does: exactly 0xc0 || 0..0 is the identity, anything else must decode to a point of G1 other than the
+ * identity.  setup_g2_96: [tau] G2 of the trusted setup (KZG_SETUP_G2_MONOMIAL[1]), 96-byte Zcash-flag compressed;
+ * it is decoded and subgroup-checked once per call on the device.
+ *
+ * out_ok[i] = verify_kzg_proof(C_i, z_i, y_i, pi_i): C, pi valid, z, y < r, and e(C - y G1, -G2) e(pi, [tau] G2 - z G2)
+ * == 1, evaluated as e(C - y G1 + z pi, -G2) e(pi, [tau] G2) == 1.  When versioned_hashes32 != NULL (n x 32 B), also
+ * versioned_hashes32[i] == 0x01 || sha256(C_i)[1:]: with it an item is the EIP-4844 point-evaluation precompile (0x0A)
+ * on the 192-byte input versioned_hash || z || y || C || pi, which returns U256(4096) || U256(r) where out_ok is 1.
+ * commitments48, proofs48: n x 48 B; zs32, ys32: n x 32 B.
+ * Everything about an item's content (a bad encoding, a point off the curve or outside G1, a non-canonical identity,
+ * z or y >= r, a wrong versioned hash, a failed pairing) is a 0 verdict, never an error.  NMSM_ERR_ARG for null
+ * pointers, n >= 2^30, and a setup_g2_96 that does not decode, is the identity or is outside G2.  n == 0 writes nothing.
+ * With profiling on, nmsm_last_timing reports k_kzg_prepare (with the one-thread setup check k_kzg_setup) in slot 0,
+ * k_bls_miller in slot 1, k_bls_final in slot 2 and their sum in NMSM_T_TOTAL. */
+int nmsm_bls12_381_kzg_verify_proof_batch(const uint8_t* commitments48, const uint8_t* zs32, const uint8_t* ys32,
+                                          const uint8_t* proofs48, const uint8_t* versioned_hashes32, uint64_t n,
+                                          const uint8_t* setup_g2_96, uint8_t* out_ok);
+
+/* out_ok[i] = verify_blob_kzg_proof(blob_i, C_i, pi_i): every blob element < r, z = compute_challenge(blob, C) (SHA-256
+ * of "FSBLOBVERIFY_V1_" || 4096 as 16 bytes big-endian || blob || C, mod r), y = the blob's polynomial at z
+ * (evaluate_polynomial_in_evaluation_form over the bit-reversed 4096-th roots of unity of 7), then the rules of
+ * nmsm_bls12_381_kzg_verify_proof_batch without a versioned hash.  blobs: n x 131072 B (4096 elements each);
+ * commitments48, proofs48: n x 48 B.  The all-zero blob with identity commitment and proof verifies.  Errors and verdict
+ * rules as for nmsm_bls12_381_kzg_verify_proof_batch.  Blobs are uploaded and evaluated 1024 at a time (128 MiB of
+ * device memory).  The first call after nmsm_init builds the domain (4096 x 32 B), kept until nmsm_shutdown.  With
+ * profiling on, nmsm_last_timing reports k_kzg_challenge in slot 0, k_kzg_eval in slot 1 (each summed over the chunks),
+ * k_kzg_prepare (with k_kzg_setup) in slot 2, k_bls_miller in slot 3, k_bls_final in slot 4 and their sum in
+ * NMSM_T_TOTAL. */
+int nmsm_bls12_381_kzg_verify_blob_batch(const uint8_t* blobs, const uint8_t* commitments48, const uint8_t* proofs48,
+                                         uint64_t n, const uint8_t* setup_g2_96, uint8_t* out_ok);
 
 /* Batched wire-format decoding on the GPU (next-row f2): encodings -> canonical affine points in the packing
  * above, ready for nmsm_msm.  secp256k1: 33-byte SEC1 compressed (weierstrass.ts:565-588); BLS12-381 G1: 48-byte

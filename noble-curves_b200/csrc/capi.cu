@@ -425,6 +425,8 @@ void nmsm_shutdown(void) {
   C.p256_g_table = nullptr;
   cudaFree(C.p384_g_table);
   C.p384_g_table = nullptr;
+  cudaFree(C.kzg_roots);
+  C.kzg_roots = nullptr;
   cudaFree(C.ed25519_b_table);
   C.ed25519_b_table = nullptr;
   for (Buf* b : {&C.ntt_data, &C.ntt_work, &C.ntt_tmp, &C.ntt_roots, &C.ntt_aux}) b->release();
@@ -980,6 +982,33 @@ int nmsm_bls12_381_aggregate_verify_batch(const uint8_t* sigs96, const uint64_t*
   if (!sigs96 || !group_off || !msg_off || !key_off || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
   return bls12_381_aggregate_verify_batch_impl(sigs96, group_off, n_checks, msgs, msg_off, keys_xy, key_off, dst,
                                                dst_len, out_ok);
+}
+
+int nmsm_bls12_381_kzg_verify_proof_batch(const uint8_t* commitments48, const uint8_t* zs32, const uint8_t* ys32,
+                                          const uint8_t* proofs48, const uint8_t* versioned_hashes32, uint64_t n,
+                                          const uint8_t* setup_g2_96, uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n must be < 2^30");
+  if (!commitments48 || !zs32 || !ys32 || !proofs48 || !setup_g2_96 || !out_ok)
+    return fail(NMSM_ERR_ARG, "null pointer");
+  return bls12_381_kzg_verify_proof_batch_impl(commitments48, zs32, ys32, proofs48, versioned_hashes32, n, setup_g2_96,
+                                               out_ok);
+}
+
+int nmsm_bls12_381_kzg_verify_blob_batch(const uint8_t* blobs, const uint8_t* commitments48, const uint8_t* proofs48,
+                                         uint64_t n, const uint8_t* setup_g2_96, uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (n == 0) return NMSM_OK;
+  if (n >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n must be < 2^30");
+  if (!blobs || !commitments48 || !proofs48 || !setup_g2_96 || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
+  return bls12_381_kzg_verify_blob_batch_impl(blobs, commitments48, proofs48, n, setup_g2_96, out_ok);
 }
 
 int nmsm_points_decode_ex(int curve, const uint8_t* enc, uint64_t n, int flags, uint8_t* out_xy, uint8_t* out_status) {

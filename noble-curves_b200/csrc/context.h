@@ -103,6 +103,7 @@ struct Context {
   uint32_t* ed25519_b_table = nullptr;    // fixed-point table of the ed25519 base point, built by the first verify_each
   uint32_t* p256_g_table = nullptr;       // fixed-point table of the P-256 generator, built by the first P-256 verify
   uint32_t* p384_g_table = nullptr;       // fixed-point table of the P-384 generator, built by the first P-384 verify
+  uint32_t* kzg_roots = nullptr;          // the EIP-4844 bit-reversed domain (Montgomery form), built by the first blob verify
   Buf ntt_data, ntt_work, ntt_tmp, ntt_roots, ntt_aux;  // NTT staging / work / output / root table (ntt.cu)
   int ntt_key_field = -1, ntt_key_bits = -1;            // which root table ntt_roots holds
   uint64_t ntt_key_gen = 0;
@@ -263,6 +264,11 @@ int bls12_381_aggregate_verify_batch_impl(const uint8_t* sigs96, const uint64_t*
                                           const uint8_t* msgs, const uint64_t* msg_off, const uint8_t* keys_xy,
                                           const uint64_t* key_off, const uint8_t* dst, uint64_t dst_len,
                                           uint8_t* out_ok);
+int bls12_381_kzg_verify_proof_batch_impl(const uint8_t* commitments48, const uint8_t* zs32, const uint8_t* ys32,
+                                          const uint8_t* proofs48, const uint8_t* versioned_hashes32, uint64_t n,
+                                          const uint8_t* setup_g2_96, uint8_t* out_ok);
+int bls12_381_kzg_verify_blob_batch_impl(const uint8_t* blobs, const uint8_t* commitments48, const uint8_t* proofs48,
+                                         uint64_t n, const uint8_t* setup_g2_96, uint8_t* out_ok);
 int decode_points_impl(int curve, const uint8_t* enc, uint64_t n, int flags, uint8_t* out_xy, uint8_t* out_status);
 int ntt_impl(int curve, void* values, int on_device, int log_n, uint64_t generator, int inverse, int brp_input,
              int brp_output);

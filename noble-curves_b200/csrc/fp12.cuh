@@ -9,6 +9,8 @@
 // The tower is a template over a policy T (field parameters, multiplication by xi, Frobenius coefficients, the curve
 // parameter x of the cyclotomic exponentiation): Bls381Tower and Bn254Tower.  The heavy operations are out of line on
 // the device (NMSM_HD_NOINLINE): one copy of each body keeps the pairing kernels' code size and ptxas time reasonable.
+// `inline` gives the host copies of the non-template ones (pairing.cuh) one definition per program, so more than one
+// translation unit can include them (inst_bls381_pairing.cu and inst_kzg.cu); the device calls stay out of line.
 #pragma once
 #include "curve_consts.cuh"
 #include "fp2.cuh"
@@ -16,7 +18,7 @@
 namespace nmsm {
 
 #if defined(__CUDACC__)
-#define NMSM_HD_NOINLINE __host__ __device__ __noinline__
+#define NMSM_HD_NOINLINE inline __host__ __device__ __noinline__
 #else
 #define NMSM_HD_NOINLINE inline
 #endif

@@ -116,8 +116,9 @@ k_bls_agg_prepare(uint32_t n, const uint8_t* __restrict__ sigs, const uint64_t* 
   if (j < n) bls_agg_prepare_body(j, sigs, group_off, group_ok, g1, g2, pre_ok);
 }
 
-namespace {
 const PairingKernels BLS_KERNELS{k_bls_miller, k_bls_final};
+
+namespace {
 
 // keys per tile of k_bls_key_tiles, and the most tiles one group is split into (bls_key_tiles)
 constexpr uint64_t BLS_KEY_TILE = 128, BLS_KEY_TILE_CAP = 256;

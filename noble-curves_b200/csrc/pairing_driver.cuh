@@ -24,6 +24,8 @@ struct PairingKernels {
   void (*final)(uint64_t j0, uint32_t cnt, const uint64_t* off, uint64_t q0, uint64_t q1, const uint32_t* W,
                 const uint32_t* carry_in, uint32_t* carry_out, const uint8_t* pre_ok, uint8_t* out_ok);
 };
+// BLS12-381's (inst_bls381_pairing.cu), also run by the KZG proof checks of inst_kzg.cu
+extern const PairingKernels BLS_KERNELS;
 
 namespace {
 // Runs one launch; with profiling on, times it with events 0-1 of slot 0 and adds the time to last_ms[slot] and to

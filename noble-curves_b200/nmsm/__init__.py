@@ -1803,6 +1803,149 @@ def _bls_verify_short_signature(signature, message, publicKey) -> bool:
 bls12_381.verifyShortSignature = _bls_verify_short_signature
 
 
+# ---- EIP-4844 KZG proofs (include/nmsm.h nmsm_bls12_381_kzg_verify_proof_batch, nmsm_bls12_381_kzg_verify_blob_batch)
+# The consensus specs' verify_kzg_proof / verify_blob_kzg_proof RAISE on malformed input (a length, a point that does
+# not decode or lies outside G1, a field element >= r); these batch forms return False for that item instead, as the
+# point-evaluation precompile fails the call.  Only the arguments' shapes and the setup point raise.
+KZG_FIELD_ELEMENTS_PER_BLOB = 4096
+KZG_BYTES_PER_BLOB = 32 * KZG_FIELD_ELEMENTS_PER_BLOB
+KZG_BLS_MODULUS = 0x73EDA753299D7D483339D80809A1D80553BDA402FFFE5BFEFFFFFFFF00000001
+POINT_EVALUATION_INPUT_BYTES = 192  # versioned_hash || z || y || commitment || proof
+# what the precompile returns on success: FIELD_ELEMENTS_PER_BLOB and BLS_MODULUS as 32-byte big-endian words
+POINT_EVALUATION_OUTPUT = KZG_FIELD_ELEMENTS_PER_BLOB.to_bytes(32, "big") + KZG_BLS_MODULUS.to_bytes(32, "big")
+
+
+def _kzg_bytes(items, width: int, name: str) -> bytes:
+    out = []
+    for x in items:
+        if not isinstance(x, (bytes, bytearray, memoryview)):
+            raise TypeError('"%s" expected bytes, got type=%s' % (name, type(x).__name__))
+        if len(x) != width:
+            raise ValueError('"%s" expected %d bytes, got length=%d' % (name, width, len(x)))
+        out.append(bytes(x))
+    return b"".join(out)
+
+
+def _kzg_scalars(items, name: str) -> bytes:
+    """z or y values as 32-byte big-endian words: ints in [0, 2^256) or 32-byte values (a value >= r is a False verdict)"""
+    out = []
+    for x in items:
+        if isinstance(x, int) and not isinstance(x, bool):
+            if not 0 <= x < 1 << 256:
+                raise ValueError('"%s" expected an integer in [0, 2^256), got %d' % (name, x))
+            x = x.to_bytes(32, "big")
+        out.append(x)
+    return _kzg_bytes(out, 32, name)
+
+
+def _kzg_setup(setup_g2) -> bytes:
+    if isinstance(setup_g2, bls12_381.G2.Point):
+        setup_g2 = _bls_g2_compress(setup_g2)
+    return _kzg_bytes([setup_g2], 96, "setup_g2")
+
+
+def kzg_verify_proof_batch(commitments, zs, ys, proofs, setup_g2) -> List[bool]:
+    """Batch form of the consensus specs' verify_kzg_proof(commitment, z, y, proof) (EIP-4844): one verdict per item.
+    Commitments and proofs are 48-byte compressed G1 encodings; z and y are ints or 32-byte big-endian values;
+    setup_g2 is [tau] G2 (KZG_SETUP_G2_MONOMIAL[1]) as 96 compressed bytes or a bls12_381.G2.Point.  Malformed items
+    are False (the spec raises); a setup point that does not decode or lies outside G2 raises NmsmError (ERR_ARG)."""
+    n = len(commitments)
+    if len(zs) != n or len(ys) != n or len(proofs) != n:
+        raise ValueError("commitments, zs, ys and proofs must have equal length")
+    args = (_kzg_bytes(commitments, 48, "commitment"), _kzg_scalars(zs, "z"), _kzg_scalars(ys, "y"),
+            _kzg_bytes(proofs, 48, "proof"))
+    setup = _kzg_setup(setup_g2)
+    if n == 0:
+        return []
+    return [b == 1 for b in kzg_verify_proof_batch_packed(*args, None, n, setup)]
+
+
+def kzg_verify_proof_batch_packed(commitments48: bytes, zs32: bytes, ys32: bytes, proofs48: bytes,
+                                  versioned_hashes32: Optional[bytes], n: int, setup_g2_96: bytes) -> bytes:
+    """The C-ABI call itself (nmsm_bls12_381_kzg_verify_proof_batch): n*48 commitment bytes, n*32 z and y bytes
+    (big-endian), n*48 proof bytes, n*32 versioned-hash bytes or None, and the 96-byte setup point.  Returns n verdict
+    bytes; raises NmsmError (with .code) on an error."""
+    if (len(commitments48) != 48 * n or len(zs32) != 32 * n or len(ys32) != 32 * n or len(proofs48) != 48 * n
+            or (versioned_hashes32 is not None and len(versioned_hashes32) != 32 * n) or len(setup_g2_96) != 96):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    vh = cp(versioned_hashes32) if versioned_hashes32 is not None else None
+    _lib.check(lib.nmsm_bls12_381_kzg_verify_proof_batch(cp(commitments48 or b"\0"), cp(zs32 or b"\0"),
+                                                         cp(ys32 or b"\0"), cp(proofs48 or b"\0"), vh, n,
+                                                         cp(setup_g2_96), out))
+    return out.raw[:n]
+
+
+def kzg_verify_blob_proof_batch(blobs, commitments, proofs, setup_g2) -> List[bool]:
+    """Batch form of the consensus specs' verify_blob_kzg_proof(blob, commitment, proof) (EIP-4844): one verdict per
+    blob.  Blobs are KZG_BYTES_PER_BLOB bytes each (4096 big-endian field elements); commitments, proofs and setup_g2
+    as for kzg_verify_proof_batch.  A blob with an element >= r, or a malformed point, is False (the spec raises)."""
+    n = len(blobs)
+    if len(commitments) != n or len(proofs) != n:
+        raise ValueError("blobs, commitments and proofs must have equal length")
+    args = (_kzg_bytes(blobs, KZG_BYTES_PER_BLOB, "blob"), _kzg_bytes(commitments, 48, "commitment"),
+            _kzg_bytes(proofs, 48, "proof"))
+    setup = _kzg_setup(setup_g2)
+    if n == 0:
+        return []
+    return [b == 1 for b in kzg_verify_blob_proof_batch_packed(*args, n, setup)]
+
+
+def kzg_verify_blob_proof_batch_packed(blobs: bytes, commitments48: bytes, proofs48: bytes, n: int,
+                                       setup_g2_96: bytes) -> bytes:
+    """The C-ABI call itself (nmsm_bls12_381_kzg_verify_blob_batch): n*131072 blob bytes, n*48 commitment and proof
+    bytes, the 96-byte setup point.  Returns n verdict bytes; raises NmsmError (with .code) on an error."""
+    if (len(blobs) != KZG_BYTES_PER_BLOB * n or len(commitments48) != 48 * n or len(proofs48) != 48 * n
+            or len(setup_g2_96) != 96):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
+    _lib.check(lib.nmsm_bls12_381_kzg_verify_blob_batch(cp(blobs or b"\0"), cp(commitments48 or b"\0"),
+                                                        cp(proofs48 or b"\0"), n, cp(setup_g2_96), out))
+    return out.raw[:n]
+
+
+def eth_point_evaluation_batch(inputs, setup_g2) -> List[bool]:
+    """Ethereum's point-evaluation precompile (0x0A, EIP-4844) over a batch: True where the precompile succeeds (and
+    returns POINT_EVALUATION_OUTPUT), False where it fails.  `inputs` is a list of byte strings or one buffer of
+    n * 192 bytes, each versioned_hash || z || y || commitment || proof.  An input that is not 192 bytes is False.  The
+    checks: versioned_hash == 0x01 || sha256(commitment)[1:], z and y < r, and verify_kzg_proof."""
+    import numpy as np
+
+    W = POINT_EVALUATION_INPUT_BYTES
+    if isinstance(inputs, (bytes, bytearray, memoryview)):
+        buf = bytes(inputs)
+        if len(buf) % W:
+            raise ValueError("a packed point-evaluation batch must be a multiple of 192 bytes, got %d" % len(buf))
+        items = np.frombuffer(buf, np.uint8).reshape(-1, W)
+        good = np.ones(len(items), bool)
+    else:
+        for x in inputs:
+            if not isinstance(x, (bytes, bytearray, memoryview)):
+                raise TypeError("point-evaluation input expected bytes, got type=%s" % type(x).__name__)
+        good = np.array([len(x) == W for x in inputs], bool)
+        items = np.zeros((len(inputs), W), np.uint8)
+        for i, x in enumerate(inputs):
+            if good[i]:
+                items[i] = np.frombuffer(bytes(x), np.uint8)
+    setup = _kzg_setup(setup_g2)
+    idx = np.flatnonzero(good)
+    out = np.zeros(len(good), bool)
+    if len(idx) == 0:
+        return out.tolist()
+    sel = items[idx]
+    col = lambda a, b: np.ascontiguousarray(sel[:, a:b]).tobytes()  # noqa: E731
+    res = kzg_verify_proof_batch_packed(col(96, 144), col(32, 64), col(64, 96), col(144, 192), col(0, 32), len(idx),
+                                        setup)
+    out[idx] = np.frombuffer(res, np.uint8) == 1
+    return out.tolist()
+
+
 # ---- bn254 pairing checks (include/nmsm.h nmsm_bn254_pairing_check_batch) and EIP-197 ecPairing ---------------------
 def bn254_pairing_check_batch(checks) -> List[bool]:
     """pairing_check_batch on bn254: checks[j] is a list of (bn254.G1.Point, bn254.G2.Point) pairs, True iff the

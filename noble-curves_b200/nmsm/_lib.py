@@ -45,6 +45,7 @@ EXPORTS = [
     "nmsm_bls12_381_pairing_check_batch", "nmsm_bls12_381_verify_batch", "nmsm_bn254_pairing_check_batch",
     "nmsm_bls12_381_hash_to_g2_batch", "nmsm_bls12_381_verify_msg_batch", "nmsm_bls12_381_aggregate_verify_batch",
     "nmsm_bls12_381_hash_to_g1_batch", "nmsm_bls12_381_short_verify_batch", "nmsm_bls12_381_short_verify_msg_batch",
+    "nmsm_bls12_381_kzg_verify_proof_batch", "nmsm_bls12_381_kzg_verify_blob_batch",
 ]
 
 
@@ -197,6 +198,10 @@ def load() -> ctypes.CDLL:
         lib.nmsm_bls12_381_hash_to_g1_batch.restype = ctypes.c_int
         lib.nmsm_bls12_381_short_verify_batch.argtypes = [u8p, u8p, u8p, ctypes.c_uint64, u8p]
         lib.nmsm_bls12_381_short_verify_batch.restype = ctypes.c_int
+        lib.nmsm_bls12_381_kzg_verify_proof_batch.argtypes = [u8p, u8p, u8p, u8p, u8p, ctypes.c_uint64, u8p, u8p]
+        lib.nmsm_bls12_381_kzg_verify_proof_batch.restype = ctypes.c_int
+        lib.nmsm_bls12_381_kzg_verify_blob_batch.argtypes = [u8p, u8p, u8p, ctypes.c_uint64, u8p, u8p]
+        lib.nmsm_bls12_381_kzg_verify_blob_batch.restype = ctypes.c_int
         lib.nmsm_bls12_381_short_verify_msg_batch.argtypes = [u8p, u8p, u8p, u8p, ctypes.c_uint64, u8p, ctypes.c_uint64,
                                                               u8p]
         lib.nmsm_bls12_381_short_verify_msg_batch.restype = ctypes.c_int
