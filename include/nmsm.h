@@ -484,6 +484,46 @@ int nmsm_bls12_381_kzg_verify_proof_batch(const uint8_t* commitments48, const ui
 int nmsm_bls12_381_kzg_verify_blob_batch(const uint8_t* blobs, const uint8_t* commitments48, const uint8_t* proofs48,
                                          uint64_t n, const uint8_t* setup_g2_96, uint8_t* out_ok);
 
+/* EIP-4844 KZG prover on BLS12-381 (next-row f16): blob_to_kzg_commitment, compute_kzg_proof and
+ * compute_blob_kzg_proof of the consensus specs (Deneb polynomial-commitments.md) over a batch of blobs, against a
+ * device-resident setup.  Each commitment and proof is g1_lincomb(bit_reversal_permutation(KZG_SETUP_G1_LAGRANGE), s)
+ * over 4096 scalars s, run as a fixed-base comb over a table of the setup points.
+ *
+ * nmsm_bls12_381_kzg_setup_create: g1_lagrange48 = KZG_SETUP_G1_LAGRANGE, 4096 x 48 B Zcash-flag compressed points in
+ * NATURAL order (the ceremony file's g1_lagrange; the library applies the bit reversal).  Every point is decoded and
+ * checked to lie in G1 on the device: one that does not decode, is the identity or lies outside G1 is NMSM_ERR_POINT
+ * with nmsm_last_error_index = its index.  Then the table d 2^(8 j) P for d in [1, 128], 32 levels j and every point
+ * is built: 1.61 GB of device memory, kept until nmsm_bls12_381_kzg_setup_free or nmsm_shutdown (after which the handle
+ * only accepts _free).  NMSM_ERR_ARG for null pointers.  With profiling on, nmsm_last_timing reports the point check
+ * in slot 0, the table build in slot 1 and their sum in NMSM_T_TOTAL.
+ *
+ * The three batch calls: blobs are n x 131072 B (4096 32-byte big-endian elements); commitments and proofs are 48-byte
+ * compressed G1 (the identity is 0xc0 || 0..0); z and y are 32-byte big-endian.  Where the spec raises (a blob element
+ * >= r, z >= r, a commitment that fails validate_kzg_g1) the item gets out_ok[i] = 0 and zero output bytes, never an
+ * error.  NMSM_ERR_ARG for null pointers, a null or unknown handle, a setup released by nmsm_shutdown and n >= 2^30.
+ * n == 0 writes nothing.  Blobs are uploaded and processed 1024 at a time (128 MiB of device memory besides the table);
+ * a proof replaces each blob's chunk by its quotient in place.
+ *
+ * nmsm_bls12_381_kzg_commit_batch: out_commitments48[i] = blob_to_kzg_commitment(blob_i).  With profiling on,
+ * nmsm_last_timing reports k_kzg_lincomb (with k_kzg_lincomb_finish) in slot 0 and in NMSM_T_TOTAL. */
+int nmsm_bls12_381_kzg_setup_create(const uint8_t* g1_lagrange48, uint64_t* out_handle);
+int nmsm_bls12_381_kzg_setup_free(uint64_t handle);
+int nmsm_bls12_381_kzg_commit_batch(uint64_t setup, const uint8_t* blobs, uint64_t n, uint8_t* out_commitments48,
+                                    uint8_t* out_ok);
+/* (out_proofs48[i], out_ys32[i]) = compute_kzg_proof(blob_i, z_i): y = f(z), q_i = (f_i - y) / (w_i - z) and, where
+ * z = w_m is on the domain, q_m = compute_quotient_eval_within_domain; the proof is the lincomb over q.  zs32: n x 32 B.
+ * With profiling on, nmsm_last_timing reports k_kzg_eval in slot 0, k_kzg_quotient in slot 1, k_kzg_lincomb (with
+ * k_kzg_lincomb_finish) in slot 2, each summed over the chunks, and their sum in NMSM_T_TOTAL. */
+int nmsm_bls12_381_kzg_compute_proof_batch(uint64_t setup, const uint8_t* blobs, const uint8_t* zs32, uint64_t n,
+                                           uint8_t* out_proofs48, uint8_t* out_ys32, uint8_t* out_ok);
+/* out_proofs48[i] = compute_blob_kzg_proof(blob_i, C_i): C_i is checked as validate_kzg_g1 does, z =
+ * compute_challenge(blob_i, C_i), then the proof of compute_kzg_proof at z.  commitments48: n x 48 B.  With
+ * profiling on, nmsm_last_timing reports k_kzg_challenge (with the commitment check) in slot 0, k_kzg_eval in slot 1,
+ * k_kzg_quotient in slot 2, k_kzg_lincomb (with k_kzg_lincomb_finish) in slot 3, each summed over the chunks, and their
+ * sum in NMSM_T_TOTAL. */
+int nmsm_bls12_381_kzg_compute_blob_proof_batch(uint64_t setup, const uint8_t* blobs, const uint8_t* commitments48,
+                                                uint64_t n, uint8_t* out_proofs48, uint8_t* out_ok);
+
 /* Batched wire-format decoding on the GPU (next-row f2): encodings -> canonical affine points in the packing
  * above, ready for nmsm_msm.  secp256k1: 33-byte SEC1 compressed (weierstrass.ts:565-588); BLS12-381 G1: 48-byte
  * Zcash-flag compressed (bls12-381.ts:377-468); BLS12-381 G2: 96-byte Zcash-flag compressed, x = c1 || c0

@@ -427,6 +427,7 @@ void nmsm_shutdown(void) {
   C.p384_g_table = nullptr;
   cudaFree(C.kzg_roots);
   C.kzg_roots = nullptr;
+  kzg_release_setups();
   cudaFree(C.ed25519_b_table);
   C.ed25519_b_table = nullptr;
   for (Buf* b : {&C.ntt_data, &C.ntt_work, &C.ntt_tmp, &C.ntt_roots, &C.ntt_aux}) b->release();
@@ -1009,6 +1010,64 @@ int nmsm_bls12_381_kzg_verify_blob_batch(const uint8_t* blobs, const uint8_t* co
   if (n >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n must be < 2^30");
   if (!blobs || !commitments48 || !proofs48 || !setup_g2_96 || !out_ok) return fail(NMSM_ERR_ARG, "null pointer");
   return bls12_381_kzg_verify_blob_batch_impl(blobs, commitments48, proofs48, n, setup_g2_96, out_ok);
+}
+
+int nmsm_bls12_381_kzg_setup_create(const uint8_t* g1_lagrange48, uint64_t* out_handle) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (!g1_lagrange48 || !out_handle) return fail(NMSM_ERR_ARG, "null pointer");
+  return bls12_381_kzg_setup_create_impl(g1_lagrange48, out_handle);
+}
+
+int nmsm_bls12_381_kzg_setup_free(uint64_t handle) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (!handle) return fail(NMSM_ERR_ARG, "null handle");
+  return bls12_381_kzg_setup_free_impl(handle);
+}
+
+// the argument checks the three provers share
+static int kzg_prove_args(uint64_t setup, const uint8_t* blobs, uint64_t n, const void* in2, const uint8_t* out48,
+                          const uint8_t* out_ok) {
+  if (!setup) return fail(NMSM_ERR_ARG, "null handle");
+  if (n >= (1ull << 30)) return fail(NMSM_ERR_ARG, "n must be < 2^30");
+  if (n && (!blobs || !in2 || !out48 || !out_ok)) return fail(NMSM_ERR_ARG, "null pointer");
+  return NMSM_OK;
+}
+
+int nmsm_bls12_381_kzg_commit_batch(uint64_t setup, const uint8_t* blobs, uint64_t n, uint8_t* out_commitments48,
+                                    uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (int r = kzg_prove_args(setup, blobs, n, blobs, out_commitments48, out_ok)) return r;
+  if (n == 0) return NMSM_OK;
+  return bls12_381_kzg_commit_batch_impl(setup, blobs, n, out_commitments48, out_ok);
+}
+
+int nmsm_bls12_381_kzg_compute_proof_batch(uint64_t setup, const uint8_t* blobs, const uint8_t* zs32, uint64_t n,
+                                           uint8_t* out_proofs48, uint8_t* out_ys32, uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (int r = kzg_prove_args(setup, blobs, n, zs32, out_proofs48, out_ok)) return r;
+  if (n && !out_ys32) return fail(NMSM_ERR_ARG, "null pointer");
+  if (n == 0) return NMSM_OK;
+  return bls12_381_kzg_compute_proof_batch_impl(setup, blobs, zs32, n, out_proofs48, out_ys32, out_ok);
+}
+
+int nmsm_bls12_381_kzg_compute_blob_proof_batch(uint64_t setup, const uint8_t* blobs, const uint8_t* commitments48,
+                                                uint64_t n, uint8_t* out_proofs48, uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int r = ensure_init()) return r;
+  g_ctx.cur = 0;
+  SLOT0_FREE();
+  if (int r = kzg_prove_args(setup, blobs, n, commitments48, out_proofs48, out_ok)) return r;
+  if (n == 0) return NMSM_OK;
+  return bls12_381_kzg_compute_blob_proof_batch_impl(setup, blobs, commitments48, n, out_proofs48, out_ok);
 }
 
 int nmsm_points_decode_ex(int curve, const uint8_t* enc, uint64_t n, int flags, uint8_t* out_xy, uint8_t* out_status) {

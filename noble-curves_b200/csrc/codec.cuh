@@ -88,6 +88,15 @@ NMSM_HD int sec1_decode_secp256k1(const uint8_t* enc, uint32_t* out_xy) {
   return sec1_decode_compressed<CurveSecp256k1>(enc, out_xy);
 }
 
+// sortBit of a canonical BLS12-381 Fp element (12 words): y is the lexicographically larger root iff 2*y >= p
+// (bls12-381.ts:347-352)
+NMSM_HD bool bls12_381_sort_bit(const uint32_t* yw) {
+  uint32_t d2[12];
+  for (int k = 11; k >= 1; k--) d2[k] = (yw[k] << 1) | (yw[k - 1] >> 31);
+  d2[0] = yw[0] << 1;  // 2y < 2^382: no overflow
+  return !Fp<FpBls381>::canonical_in_range(d2);
+}
+
 NMSM_HD int zcash_decode_bls12_381_g1(const uint8_t* enc, uint32_t* out_xy) {
   using F = Fp<FpBls381>;
   const bool compressed = (enc[0] >> 7) & 1, infinity = (enc[0] >> 6) & 1, sort = (enc[0] >> 5) & 1;
@@ -111,14 +120,9 @@ NMSM_HD int zcash_decode_bls12_381_g1(const uint8_t* enc, uint32_t* out_xy) {
   bool ok;
   F y = fp_sqrt_3mod4<FpBls381>(sqr(x) * x + b, ok);
   if (!ok) return 0;
-  // sortBit: y is the lexicographically larger root iff 2*y >= p  (bls12-381.ts:347-352)
   uint32_t yw[12];
   y.to_canonical(yw);
-  uint32_t d2[12];
-  for (int k = 11; k >= 1; k--) d2[k] = (yw[k] << 1) | (yw[k - 1] >> 31);
-  d2[0] = yw[0] << 1;  // 2y < 2^382: no overflow
-  const bool larger = !F::canonical_in_range(d2);
-  if (larger != sort) {
+  if (bls12_381_sort_bit(yw) != sort) {
     y = -y;
     y.to_canonical(yw);
   }

@@ -269,6 +269,15 @@ int bls12_381_kzg_verify_proof_batch_impl(const uint8_t* commitments48, const ui
                                           const uint8_t* setup_g2_96, uint8_t* out_ok);
 int bls12_381_kzg_verify_blob_batch_impl(const uint8_t* blobs, const uint8_t* commitments48, const uint8_t* proofs48,
                                          uint64_t n, const uint8_t* setup_g2_96, uint8_t* out_ok);
+int bls12_381_kzg_setup_create_impl(const uint8_t* g1_lagrange48, uint64_t* out_handle);
+int bls12_381_kzg_setup_free_impl(uint64_t handle);
+void kzg_release_setups();  // nmsm_shutdown: frees every setup table (the handles stay until nmsm_bls12_381_kzg_setup_free)
+int bls12_381_kzg_commit_batch_impl(uint64_t setup, const uint8_t* blobs, uint64_t n, uint8_t* out_commitments48,
+                                    uint8_t* out_ok);
+int bls12_381_kzg_compute_proof_batch_impl(uint64_t setup, const uint8_t* blobs, const uint8_t* zs32, uint64_t n,
+                                           uint8_t* out_proofs48, uint8_t* out_ys32, uint8_t* out_ok);
+int bls12_381_kzg_compute_blob_proof_batch_impl(uint64_t setup, const uint8_t* blobs, const uint8_t* commitments48,
+                                                uint64_t n, uint8_t* out_proofs48, uint8_t* out_ok);
 int decode_points_impl(int curve, const uint8_t* enc, uint64_t n, int flags, uint8_t* out_xy, uint8_t* out_status);
 int ntt_impl(int curve, void* values, int on_device, int log_n, uint64_t generator, int inverse, int brp_input,
              int brp_output);

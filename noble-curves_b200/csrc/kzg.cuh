@@ -16,6 +16,10 @@
 // 0xc0 || 0..0 is allowed, anything else must decode and lie in G1), range checks of z and y, the optional versioned
 // hash, and Q; the Miller and final kernels are the BLS pairing checks' (pairing.cuh), two pairs per check.
 //
+// The prover (SURVEY §8 row f16; blob_to_kzg_commitment, compute_kzg_proof, compute_blob_kzg_proof) is at the end: the
+// setup table of the Lagrange points, the comb lincomb over it, the quotient by Montgomery's batch inversion, and the
+// G1 compression of the results.
+//
 // Bodies are host/device so tests/hostemu can run them; the *_serial statements are what the kernels compute.
 #pragma once
 #include "ecdsa_verify.cuh"
@@ -59,6 +63,13 @@ NMSM_HD KzgFr kzg_pow(const KzgFr& a, const uint32_t* e, int bits) {
   return r;
 }
 
+// i with its 12 bits reversed: the index map of bit_reversal_permutation over 4096 elements (an involution)
+NMSM_HD uint32_t kzg_brp(uint32_t i) {
+  uint32_t j = 0;
+  for (int b = 0; b < 12; b++) j |= ((i >> b) & 1u) << (11 - b);
+  return j;
+}
+
 // w_i = omega^brp(i) in Montgomery form, omega = 7^((r - 1) / 4096): the spec's bit-reversed domain
 NMSM_HD KzgFr kzg_root(uint32_t i) {
   uint32_t e[8], seven[8] = {7, 0, 0, 0, 0, 0, 0, 0};
@@ -67,8 +78,7 @@ NMSM_HD KzgFr kzg_root(uint32_t i) {
     e[k] = (lo >> 12) | (hi << 20);
   }
   const KzgFr omega = kzg_pow(KzgFr::from_canonical(seven), e, 243);
-  uint32_t j = 0;
-  for (int b = 0; b < 12; b++) j |= ((i >> b) & 1u) << (11 - b);
+  const uint32_t j = kzg_brp(i);
   return kzg_pow(omega, &j, 12);
 }
 
@@ -254,6 +264,173 @@ NMSM_HD void kzg_prepare_serial(uint32_t n, const uint8_t* commitments48, const 
     const bool ok = kzg_prepare_body(i, commitments48, zs32, ys32, proofs48, vhs32, item_ok, q, pi);
     kzg_store_pairs(i, ok, q, inv(ok ? KzgG::inv_target(q) : BlsF::one()), pi, setup_xy, g1, g2, pre_ok);
   }
+}
+
+// ---- the prover: blob_to_kzg_commitment, compute_kzg_proof, compute_blob_kzg_proof -----------------------------------
+// Every commitment and proof is g1_lincomb(bit_reversal_permutation(KZG_SETUP_G1_LAGRANGE), s) over 4096 scalars s:
+// the blob's elements or the quotient's.  The setup table holds d 2^(b j) P_p for every setup point P_p (already in
+// bit-reversed order), level j < ceil(256 / b) and d in [1, 2^(b-1)], level-major: entry (j, p, d) at
+// ((j * 4096 + p) 2^(b-1) + d - 1) * 24 words in the prepared affine layout.  A lincomb is then one gathered mixed
+// addition per point and level (table_walk_acc over the signed b-bit digits of s_p) and no doubling.
+using KzgCv = CurveBls381G1Any;
+static constexpr int KZG_COMB_BITS = 8;  // b: 4096 x 32 levels x 128 entries x 96 B = 1.61 GB (DESIGN.md §4h)
+
+template <int BITS = KZG_COMB_BITS>
+NMSM_HD constexpr uint64_t kzg_table_bytes(uint32_t npts) {
+  return (uint64_t)point_table_levels<KzgCv, BITS>() * npts * (1u << (BITS - 1)) * KzgG::AFF_WORDS * 4;
+}
+
+// setup point i (natural order, 48-byte compressed) -> canonical affine words at position brp(i) of `xy` (k_prepare
+// then converts them to the prepared layout); false when it does not decode, is the identity or lies outside G1
+NMSM_HD bool kzg_setup_point_body(uint32_t i, const uint8_t* g1_48, uint32_t* xy) {
+  return kzg_decode_g1(g1_48 + 48 * (size_t)i, xy + 24 * (size_t)kzg_brp(i)) == 1;
+}
+
+// level 0, entry t = p 2^(b-1) + d - 1: d P_p (table_base_body per point)
+template <int BITS = KZG_COMB_BITS>
+NMSM_HD void kzg_table_base_body(uint32_t t, const uint32_t* aff, uint32_t* tbl) {
+  constexpr uint32_t HALF = 1u << (BITS - 1);
+  const uint32_t p = t / HALF;
+  table_base_body<KzgCv, BITS>(t % HALF, aff + (size_t)p * KzgG::AFF_WORDS, tbl + (size_t)p * HALF * KzgG::AFF_WORDS);
+}
+
+// lane t of S: acc += s_p P_p over the points p = t, t + S, ... < NPTS, s_p the 32-byte big-endian scalars; bad when
+// one of them is >= r
+template <int BITS = KZG_COMB_BITS, uint32_t NPTS = KZG_N>
+NMSM_HD void kzg_lincomb_lane(uint32_t t, uint32_t S, const uint8_t* scalars_be, const uint32_t* tbl, KzgG::Acc& acc,
+                              bool& bad) {
+  constexpr size_t HALF = 1u << (BITS - 1);
+  for (uint32_t p = t; p < NPTS; p += S) {
+    uint32_t s[8];
+    kzg_load_fr(s, scalars_be + 32 * (size_t)p);
+    bad |= !KzgFr::canonical_in_range(s);
+    table_walk_acc<KzgCv, BITS, NPTS * HALF>(tbl + p * HALF * KzgG::AFF_WORDS, s, acc);
+  }
+}
+
+// The 48-byte Zcash-flag compressed encoding of a canonical affine point (24 words): x big-endian with 0x80, plus 0x20
+// when y > (p - 1) / 2; the identity is 0xc0 || 0..0
+NMSM_HD void kzg_g1_compress(const uint32_t* xy, bool inf, uint8_t* out48) {
+  for (int k = 0; k < 48; k++) out48[k] = 0;
+  if (inf) {
+    out48[0] = 0xc0;
+    return;
+  }
+  for (int k = 0; k < 12; k++)
+    for (int j = 0; j < 4; j++) out48[47 - 4 * k - j] = (uint8_t)(xy[k] >> (8 * j));
+  out48[0] |= bls12_381_sort_bit(xy + 12) ? 0xa0 : 0x80;
+}
+
+// the sum of P accumulators stored one after another
+NMSM_HD_NOINLINE KzgG::Acc kzg_sum_parts(const uint32_t* parts, uint32_t P) {
+  KzgG::Acc acc = KzgG::identity();
+  for (uint32_t k = 0; k < P; k++) nl_add<KzgG>(acc, load_acc<KzgG>(parts + (size_t)k * KzgG::ACC_WORDS));
+  return acc;
+}
+
+// a lincomb's accumulator, normalised with zi = 1 / inv_target(acc), compressed
+NMSM_HD_NOINLINE void kzg_store_g1(const KzgG::Acc& acc, const KzgG::Field& zi, uint8_t* out48) {
+  uint32_t xy[24], inf;
+  KzgG::to_affine_canonical_with_inv(acc, zi, xy, &inf);
+  kzg_g1_compress(xy, inf != 0, out48);
+}
+
+// serial statement of k_kzg_lincomb + k_kzg_lincomb_finish for blob i (S lanes one after another)
+template <int BITS = KZG_COMB_BITS, uint32_t NPTS = KZG_N>
+NMSM_HD void kzg_lincomb_serial(uint32_t i, uint32_t S, const uint8_t* scalars_be, const uint32_t* tbl, uint8_t* out48,
+                                uint8_t* item_ok) {
+  KzgG::Acc sum = KzgG::identity();
+  bool bad = false;
+  for (uint32_t t = 0; t < S; t++) {
+    KzgG::Acc acc = KzgG::identity();
+    kzg_lincomb_lane<BITS, NPTS>(t, S, scalars_be + (size_t)i * 32 * NPTS, tbl, acc, bad);
+    nl_add<KzgG>(sum, acc);
+  }
+  if (bad) item_ok[i] = 0;
+  kzg_store_g1(sum, inv(KzgG::inv_target(sum)), out48 + 48 * (size_t)i);
+}
+
+// ---- compute_kzg_proof_impl's quotient q_i = (f_i - y) / (w_i - z), in place of the blob ------------------------------
+// z and y of blob i in Montgomery form; false when the blob failed its range vote (item_ok) or z >= r
+NMSM_HD bool kzg_quotient_start(uint32_t i, const uint8_t* zs32, const uint8_t* ys32, const uint8_t* item_ok, KzgFr& z,
+                                KzgFr& y) {
+  uint32_t zw[8], yw[8];
+  kzg_load_fr(zw, zs32 + (size_t)i * 32);
+  kzg_load_fr(yw, ys32 + (size_t)i * 32);
+  if (!item_ok[i] || !KzgFr::canonical_in_range(zw)) return false;
+  z = KzgFr::from_canonical(zw);
+  y = KzgFr::from_canonical(yw);
+  return true;
+}
+
+// Montgomery's batch inversion over lane t's elements e_j = t + 256 j.  Forward: d_j = w_j - z (a zero d_m, z = w_m,
+// taken as 1 and m reported in hit, as kzg_eval_lane does), P_j = d_0 ... d_j, and element e_j overwritten by
+// P_(j-1) (f_j - y) as 8 Montgomery words.  Returns P_15.
+NMSM_HD KzgFr kzg_quotient_fwd(uint32_t t, uint8_t* blob, const KzgFr& z, const KzgFr& y, const uint32_t* roots,
+                               int& hit) {
+  KzgFr pre = KzgFr::one();
+  for (int j = 0; j < KZG_PER_LANE; j++) {
+    const uint32_t e = t + KZG_EVAL_THREADS * j;
+    uint32_t fw[8];
+    kzg_load_fr(fw, blob + 32 * (size_t)e);
+    KzgFr w;
+    load_words<8>(w.v, roots + 8 * (size_t)e);
+    KzgFr d = w - z;
+    if (d.is_zero()) {
+      hit = (int)e;
+      d = KzgFr::one();
+    }
+    const KzgFr m = pre * (KzgFr::from_canonical(fw) - y);
+    store_words<8>(reinterpret_cast<uint32_t*>(blob + 32 * (size_t)e), m.v);
+    pre = pre * d;
+  }
+  return pre;
+}
+
+// Back-sweep from ri = 1 / P_15: q_j = P_(j-1) (f_j - y) / P_j, then 1 / P_(j-1) = d_j / P_j; q_j stored as 32
+// big-endian bytes.  With `sum`: returns sum_j q_j w_j, the term of the within-domain quotient.
+NMSM_HD KzgFr kzg_quotient_back(uint32_t t, uint8_t* blob, const KzgFr& z, const uint32_t* roots, KzgFr ri, bool sum) {
+  KzgFr acc = KzgFr::zero();
+  for (int j = KZG_PER_LANE - 1; j >= 0; j--) {
+    const uint32_t e = t + KZG_EVAL_THREADS * j;
+    KzgFr m, w;
+    load_words_rw<8>(m.v, reinterpret_cast<const uint32_t*>(blob + 32 * (size_t)e));
+    load_words<8>(w.v, roots + 8 * (size_t)e);
+    KzgFr d = w - z;
+    if (d.is_zero()) d = KzgFr::one();
+    const KzgFr q = m * ri;
+    ri = ri * d;
+    if (sum) acc = acc + q * w;
+    uint32_t qw[8];
+    q.to_canonical(qw);
+    kzg_store_fr(blob + 32 * (size_t)e, qw);
+  }
+  return acc;
+}
+
+// z = w_m: q_m = compute_quotient_eval_within_domain(z, f, y) = sum_(i != m) (f_i - y) w_i / (z (z - w_i))
+// = -(1 / z) sum_i q_i w_i (the back-sweep left q_m = 0, since y = f_m)
+NMSM_HD void kzg_quotient_in_domain(uint8_t* blob, int m, const KzgFr& z, const KzgFr& sum) {
+  uint32_t qw[8];
+  (-(sum * inv(z))).to_canonical(qw);
+  kzg_store_fr(blob + 32 * (size_t)m, qw);
+}
+
+// serial statement of k_kzg_quotient for blob i (one inversion per lane instead of one per warp)
+NMSM_HD void kzg_quotient_serial(uint32_t i, uint8_t* blobs, const uint8_t* zs32, const uint8_t* ys32,
+                                 const uint32_t* roots, uint8_t* item_ok) {
+  uint8_t* blob = blobs + (size_t)i * KZG_BLOB_BYTES;
+  KzgFr z, y;
+  if (!kzg_quotient_start(i, zs32, ys32, item_ok, z, y)) {
+    item_ok[i] = 0;
+    return;
+  }
+  int hit = -1;
+  KzgFr pre[KZG_EVAL_THREADS];
+  for (uint32_t t = 0; t < KZG_EVAL_THREADS; t++) pre[t] = kzg_quotient_fwd(t, blob, z, y, roots, hit);
+  KzgFr sum = KzgFr::zero();
+  for (uint32_t t = 0; t < KZG_EVAL_THREADS; t++) sum = sum + kzg_quotient_back(t, blob, z, roots, inv(pre[t]), hit >= 0);
+  if (hit >= 0) kzg_quotient_in_domain(blob, hit, z, sum);
 }
 
 }  // namespace nmsm

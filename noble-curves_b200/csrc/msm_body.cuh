@@ -775,6 +775,34 @@ NMSM_HD void table_base_body(uint32_t i, const uint32_t* p_aff, uint32_t* level0
   store_words<G::AFF_WORDS>(level0 + (size_t)i * G::AFF_WORDS, reinterpret_cast<const uint32_t*>(&a));
 }
 
+// acc += s * P by the signed BITS-bit digit walk: level w of the table holds d * 2^(BITS w) * P for d in [1, 2^(BITS-1)]
+// at tbl + (w * STRIDE + d - 1) * AFF_WORDS; s has scalar_words<Fn>() words.  One gathered mixed addition per non-zero
+// digit and no doublings.  A nmsm_point_table_* table holds one point (STRIDE = 2^(BITS-1)); the EIP-4844 setup table
+// (kzg.cuh) interleaves its points within each level.
+template <class Cv, int BITS, size_t STRIDE>
+NMSM_HD void table_walk_acc(const uint32_t* tbl, const uint32_t* s, typename Cv::G::Acc& acc) {
+  using G = typename Cv::G;
+  constexpr uint32_t HALF = 1u << (BITS - 1);
+  constexpr int SW = scalar_words<typename Cv::Fn>();
+  uint32_t carry = 0;
+  constexpr int LEVELS = point_table_levels<Cv, BITS>();
+  for (int w = 0; w < LEVELS; w++) {
+    uint32_t v = scalar_bits(s, w * BITS, BITS, SW) + carry;
+    carry = 0;
+    bool neg = false;
+    if (v > HALF) {
+      v = (1u << BITS) - v;
+      neg = true;
+      carry = 1;
+    }
+    if (v != 0) {
+      typename G::Affine a = load_aff<G>(tbl + ((size_t)w * STRIDE + (v - 1)) * G::AFF_WORDS);
+      a = G::cneg(a, neg);
+      nl_madd<G>(acc, a);
+    }
+  }
+}
+
 // k * P from the table as an un-normalised accumulator; scalars are scalar_words<Fn>() words each.  Returns false (and records the index) for a scalar
 // outside Point.multiply's range 1 <= k < n (allow_zero: multiplyUnsafe's 0 <= k < n).
 template <class Cv, int BITS = PT_BITS>
@@ -792,23 +820,7 @@ NMSM_HD bool table_mul_body(uint32_t i, const uint32_t* tbl, const uint32_t* sca
     atomic_min_u32(&err[1], i);
     return false;
   }
-  uint32_t carry = 0;
-  constexpr int LEVELS = point_table_levels<Cv, BITS>();
-  for (int w = 0; w < LEVELS; w++) {
-    uint32_t v = scalar_bits(s, w * BITS, BITS, SW) + carry;
-    carry = 0;
-    bool neg = false;
-    if (v > HALF) {
-      v = (1u << BITS) - v;
-      neg = true;
-      carry = 1;
-    }
-    if (v != 0) {
-      typename G::Affine a = load_aff<G>(tbl + ((size_t)w * HALF + (v - 1)) * G::AFF_WORDS);
-      a = G::cneg(a, neg);
-      nl_madd<G>(acc, a);
-    }
-  }
+  table_walk_acc<Cv, BITS, HALF>(tbl, s, acc);
   return true;
 }
 

@@ -17,7 +17,7 @@ argument shapes.  Nothing here imports `oracle/`.
 from __future__ import annotations
 
 import ctypes
-from typing import List, Optional, Sequence
+from typing import List, Optional, Sequence, Tuple
 
 from . import _lib
 from ._lib import NmsmError, PlanInfo, TIMING_NAMES, init  # noqa: F401
@@ -1944,6 +1944,112 @@ def eth_point_evaluation_batch(inputs, setup_g2) -> List[bool]:
                                         setup)
     out[idx] = np.frombuffer(res, np.uint8) == 1
     return out.tolist()
+
+
+class KzgSetup:
+    """Device-resident EIP-4844 trusted setup for the prover (nmsm_bls12_381_kzg_setup_create): KZG_SETUP_G1_LAGRANGE
+    as 4096 x 48 compressed bytes (one buffer or a list), in natural order as the ceremony file lists g1_lagrange.  The
+    points are checked to lie in G1 (a bad one raises ValueError; its NmsmError cause carries ERR_POINT and the index)
+    and a 1.61 GB table of them is built on the device, freed by close().
+
+    The batch methods are the consensus specs' blob_to_kzg_commitment, compute_kzg_proof and compute_blob_kzg_proof.
+    Where the spec raises (a blob element >= r, z >= r, a commitment that fails validate_kzg_g1) the item is None."""
+
+    def __init__(self, g1_lagrange):
+        self.handle = 0
+        if isinstance(g1_lagrange, (bytes, bytearray, memoryview)):
+            buf = bytes(g1_lagrange)
+        else:
+            buf = _kzg_bytes(g1_lagrange, 48, "g1_lagrange")
+        if len(buf) != 48 * KZG_FIELD_ELEMENTS_PER_BLOB:
+            raise ValueError("g1_lagrange expected %d points of 48 bytes, got %d bytes"
+                             % (KZG_FIELD_ELEMENTS_PER_BLOB, len(buf)))
+        _lib.ensure_init()
+        self._lib = _lib.load()
+        h = ctypes.c_uint64(0)
+        try:
+            _lib.check(self._lib.nmsm_bls12_381_kzg_setup_create(_kzg_cp(buf), ctypes.byref(h)))
+        except NmsmError as e:
+            _raise_mapped(e)
+        self.handle = h.value
+
+    def blob_to_kzg_commitment_batch_packed(self, blobs: bytes, n: int):
+        """The C-ABI call (nmsm_bls12_381_kzg_commit_batch): n*131072 blob bytes -> (n*48 commitment bytes, n ok
+        bytes); raises NmsmError on an error."""
+        _kzg_check_packed(blobs, n)
+        out, ok = ctypes.create_string_buffer(max(48 * n, 1)), ctypes.create_string_buffer(max(n, 1))
+        _lib.check(self._lib.nmsm_bls12_381_kzg_commit_batch(self.handle, _kzg_cp(blobs), n, out, ok))
+        return out.raw[:48 * n], ok.raw[:n]
+
+    def compute_kzg_proof_batch_packed(self, blobs: bytes, zs32: bytes, n: int):
+        """The C-ABI call (nmsm_bls12_381_kzg_compute_proof_batch): n*131072 blob bytes and n*32 big-endian z bytes ->
+        (n*48 proof bytes, n*32 y bytes, n ok bytes); raises NmsmError on an error."""
+        _kzg_check_packed(blobs, n, zs32, 32)
+        out, ys = ctypes.create_string_buffer(max(48 * n, 1)), ctypes.create_string_buffer(max(32 * n, 1))
+        ok = ctypes.create_string_buffer(max(n, 1))
+        _lib.check(self._lib.nmsm_bls12_381_kzg_compute_proof_batch(self.handle, _kzg_cp(blobs), _kzg_cp(zs32), n, out,
+                                                                    ys, ok))
+        return out.raw[:48 * n], ys.raw[:32 * n], ok.raw[:n]
+
+    def compute_blob_kzg_proof_batch_packed(self, blobs: bytes, commitments48: bytes, n: int):
+        """The C-ABI call (nmsm_bls12_381_kzg_compute_blob_proof_batch): n*131072 blob bytes and n*48 commitment
+        bytes -> (n*48 proof bytes, n ok bytes); raises NmsmError on an error."""
+        _kzg_check_packed(blobs, n, commitments48, 48)
+        out, ok = ctypes.create_string_buffer(max(48 * n, 1)), ctypes.create_string_buffer(max(n, 1))
+        _lib.check(self._lib.nmsm_bls12_381_kzg_compute_blob_proof_batch(self.handle, _kzg_cp(blobs),
+                                                                         _kzg_cp(commitments48), n, out, ok))
+        return out.raw[:48 * n], ok.raw[:n]
+
+    def blob_to_kzg_commitment_batch(self, blobs) -> List[Optional[bytes]]:
+        """blob_to_kzg_commitment for each blob: 48 compressed bytes, or None for a blob with an element >= r"""
+        n = len(blobs)
+        if n == 0:
+            return []
+        out, ok = self.blob_to_kzg_commitment_batch_packed(_kzg_bytes(blobs, KZG_BYTES_PER_BLOB, "blob"), n)
+        return [out[48 * i:48 * i + 48] if ok[i] == 1 else None for i in range(n)]
+
+    def compute_kzg_proof_batch(self, blobs, zs) -> List[Optional[Tuple[bytes, bytes]]]:
+        """compute_kzg_proof(blob, z) for each pair: (48-byte proof, 32-byte big-endian y), or None where the spec
+        raises.  z is an int in [0, 2^256) or 32 big-endian bytes."""
+        n = len(blobs)
+        if len(zs) != n:
+            raise ValueError("blobs and zs must have equal length")
+        args = (_kzg_bytes(blobs, KZG_BYTES_PER_BLOB, "blob"), _kzg_scalars(zs, "z"))
+        if n == 0:
+            return []
+        out, ys, ok = self.compute_kzg_proof_batch_packed(*args, n)
+        return [(out[48 * i:48 * i + 48], ys[32 * i:32 * i + 32]) if ok[i] == 1 else None for i in range(n)]
+
+    def compute_blob_kzg_proof_batch(self, blobs, commitments) -> List[Optional[bytes]]:
+        """compute_blob_kzg_proof(blob, commitment) for each pair: the 48-byte proof, or None where the spec raises"""
+        n = len(blobs)
+        if len(commitments) != n:
+            raise ValueError("blobs and commitments must have equal length")
+        args = (_kzg_bytes(blobs, KZG_BYTES_PER_BLOB, "blob"), _kzg_bytes(commitments, 48, "commitment"))
+        if n == 0:
+            return []
+        out, ok = self.compute_blob_kzg_proof_batch_packed(*args, n)
+        return [out[48 * i:48 * i + 48] if ok[i] == 1 else None for i in range(n)]
+
+    def close(self):
+        if self.handle:
+            self._lib.nmsm_bls12_381_kzg_setup_free(self.handle)
+            self.handle = 0
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _kzg_cp(b: bytes):
+    return ctypes.cast(ctypes.c_char_p(b or b"\0"), ctypes.c_void_p)
+
+
+def _kzg_check_packed(blobs: bytes, n: int, other: bytes = b"", width: int = 0):
+    if len(blobs) != KZG_BYTES_PER_BLOB * n or len(other) != width * n:
+        raise ValueError("packed arrays do not match n")
 
 
 # ---- bn254 pairing checks (include/nmsm.h nmsm_bn254_pairing_check_batch) and EIP-197 ecPairing ---------------------

@@ -46,6 +46,8 @@ EXPORTS = [
     "nmsm_bls12_381_hash_to_g2_batch", "nmsm_bls12_381_verify_msg_batch", "nmsm_bls12_381_aggregate_verify_batch",
     "nmsm_bls12_381_hash_to_g1_batch", "nmsm_bls12_381_short_verify_batch", "nmsm_bls12_381_short_verify_msg_batch",
     "nmsm_bls12_381_kzg_verify_proof_batch", "nmsm_bls12_381_kzg_verify_blob_batch",
+    "nmsm_bls12_381_kzg_setup_create", "nmsm_bls12_381_kzg_setup_free", "nmsm_bls12_381_kzg_commit_batch",
+    "nmsm_bls12_381_kzg_compute_proof_batch", "nmsm_bls12_381_kzg_compute_blob_proof_batch",
 ]
 
 
@@ -202,6 +204,18 @@ def load() -> ctypes.CDLL:
         lib.nmsm_bls12_381_kzg_verify_proof_batch.restype = ctypes.c_int
         lib.nmsm_bls12_381_kzg_verify_blob_batch.argtypes = [u8p, u8p, u8p, ctypes.c_uint64, u8p, u8p]
         lib.nmsm_bls12_381_kzg_verify_blob_batch.restype = ctypes.c_int
+        lib.nmsm_bls12_381_kzg_setup_create.argtypes = [u8p, ctypes.POINTER(ctypes.c_uint64)]
+        lib.nmsm_bls12_381_kzg_setup_create.restype = ctypes.c_int
+        lib.nmsm_bls12_381_kzg_setup_free.argtypes = [ctypes.c_uint64]
+        lib.nmsm_bls12_381_kzg_setup_free.restype = ctypes.c_int
+        lib.nmsm_bls12_381_kzg_commit_batch.argtypes = [ctypes.c_uint64, u8p, ctypes.c_uint64, u8p, u8p]
+        lib.nmsm_bls12_381_kzg_commit_batch.restype = ctypes.c_int
+        lib.nmsm_bls12_381_kzg_compute_proof_batch.argtypes = [ctypes.c_uint64, u8p, u8p, ctypes.c_uint64, u8p, u8p,
+                                                               u8p]
+        lib.nmsm_bls12_381_kzg_compute_proof_batch.restype = ctypes.c_int
+        lib.nmsm_bls12_381_kzg_compute_blob_proof_batch.argtypes = [ctypes.c_uint64, u8p, u8p, ctypes.c_uint64, u8p,
+                                                                    u8p]
+        lib.nmsm_bls12_381_kzg_compute_blob_proof_batch.restype = ctypes.c_int
         lib.nmsm_bls12_381_short_verify_msg_batch.argtypes = [u8p, u8p, u8p, u8p, ctypes.c_uint64, u8p, ctypes.c_uint64,
                                                               u8p]
         lib.nmsm_bls12_381_short_verify_msg_batch.restype = ctypes.c_int
