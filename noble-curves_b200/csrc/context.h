@@ -181,16 +181,8 @@ inline int check_offsets(const uint64_t* off, const char* name, uint64_t n) {
   return NMSM_OK;
 }
 
-// with profiling on: the two kernels of a per-signature verify (events 0-1-2 of the slot) in timing slots 0, 1 and
-// NMSM_T_TOTAL
-inline void record_verify_timing(Context& X, Slot& C) {
-  if (!X.profiling) return;
-  memset(X.last_ms, 0, sizeof(X.last_ms));
-  cudaEventElapsedTime(&X.last_ms[0], C.ev[0], C.ev[1]);
-  cudaEventElapsedTime(&X.last_ms[1], C.ev[1], C.ev[2]);
-  cudaEventElapsedTime(&X.last_ms[NMSM_T_TOTAL], C.ev[0], C.ev[2]);
-  (void)cudaGetLastError();
-}
+// the size of one piece of a scratch layout, rounded up so that the next piece starts 256-byte aligned
+inline uint64_t al256(uint64_t x) { return (x + 255) & ~255ull; }
 
 inline int ensure_init() {
   if (g_ctx.ready) return NMSM_OK;

@@ -875,6 +875,52 @@ static int run_mul_batch(const uint8_t* pts, const uint8_t* scalars, uint64_t n,
 }
 };
 
+// The fixed-point table of a curve's generator in *slot (a Context table pointer): d * 2^(16 j) * G, the table the
+// per-signature check kernels walk.  Built by the first verify after nmsm_init, freed by nmsm_shutdown.  GConsts: the
+// curve's canonical GX / GY words.
+template <class Cv, class GConsts>
+int ensure_g_table(uint32_t** slot) {
+  if (*slot) return NMSM_OK;
+  constexpr int FW = Cv::G::Field::LIMBS;
+  uint32_t g_xy[2 * FW];
+  for (int k = 0; k < FW; k++) {
+    g_xy[k] = GConsts::GX(k);
+    g_xy[FW + k] = GConsts::GY(k);
+  }
+  int levels = 0;
+  return Engine<Cv>::build_point_table((const uint8_t*)g_xy, slot, &levels);
+}
+
+// The launches and read-back of a two-kernel per-signature verify on slot 0's stream, after its inputs are uploaded:
+// reset the check kernel's 8-byte error word, run prepare() and check(), copy out_bytes of d_out (recovery's keys or
+// address words) and the n verdicts back and synchronise.  With profiling on, the two kernels (events 0-1-2 of the
+// slot) land in timing slots 0, 1 and NMSM_T_TOTAL.
+template <class Prepare, class Check>
+int verify_launch(unsigned int* d_err, Prepare prepare, Check check, const uint8_t* d_ok, uint8_t* out_ok, uint64_t n,
+                  const void* d_out = nullptr, void* out = nullptr, uint64_t out_bytes = 0) {
+  Context& X = g_ctx;
+  Slot& C = X.slot[0];
+  cudaStream_t st = C.stream;
+  CK(cudaMemsetAsync(d_err, 0xff, 8, st));
+  EV(0);
+  prepare();
+  EV(1);
+  check();
+  EV(2);
+  CK(cudaGetLastError());
+  if (out_bytes) CK(cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(out_ok, d_ok, n, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (X.profiling) {
+    memset(X.last_ms, 0, sizeof(X.last_ms));
+    cudaEventElapsedTime(&X.last_ms[0], C.ev[0], C.ev[1]);
+    cudaEventElapsedTime(&X.last_ms[1], C.ev[1], C.ev[2]);
+    cudaEventElapsedTime(&X.last_ms[NMSM_T_TOTAL], C.ev[0], C.ev[2]);
+    (void)cudaGetLastError();
+  }
+  return NMSM_OK;
+}
+
 
 #define NMSM_DEFINE_ENGINE(FN, CURVE)                                                          \
   const EngineVTable* FN() {                                                                   \

@@ -74,17 +74,14 @@ int ed25519_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uin
     return NMSM_OK;
   }
   if (2 * n + 1 >= (1ull << 31)) return fail(NMSM_ERR_ARG, "batch too large");
-  // the offsets drive device reads of `msgs`: they must start at 0 and never decrease
-  if (msg_off[0] != 0) return fail(NMSM_ERR_ARG, "msg_off[0] must be 0");
-  for (uint64_t i = 0; i < n; i++)
-    if (msg_off[i + 1] < msg_off[i]) return fail(NMSM_ERR_ARG, "msg_off must be non-decreasing (index " + std::to_string(i + 1) + ")", (long long)(i + 1));
+  if (int r = check_offsets(msg_off, "msg_off", n)) return r;
   const uint64_t msg_bytes = msg_off[n];
   const uint64_t terms = 2 * n + 1;
-  // scratch layout in one buffer (16-byte aligned pieces)
-  auto al = [](uint64_t x) { return (x + 255) & ~255ull; };
-  const uint64_t o_sig = 0, o_pk = o_sig + al(64 * n), o_msg = o_pk + al(32 * n), o_off = o_msg + al(msg_bytes + 16),
-                 o_z = o_off + al(8 * (n + 1)), o_pts = o_z + al(16 * n), o_sc = o_pts + al(64 * terms),
-                 o_zs = o_sc + al(32 * terms), o_misc = o_zs + al(32 * n), total = o_misc + 1024;
+  // scratch layout in one buffer
+  const uint64_t o_sig = 0, o_pk = o_sig + al256(64 * n), o_msg = o_pk + al256(32 * n),
+                 o_off = o_msg + al256(msg_bytes + 16), o_z = o_off + al256(8 * (n + 1)), o_pts = o_z + al256(16 * n),
+                 o_sc = o_pts + al256(64 * terms), o_zs = o_sc + al256(32 * terms), o_misc = o_zs + al256(32 * n),
+                 total = o_misc + 1024;
   CK(X.ed_scratch.ensure(total));
   uint8_t* base = (uint8_t*)X.ed_scratch.p;
   cudaStream_t st = C.stream;
@@ -140,56 +137,41 @@ k_ed_verify_check(uint32_t n, const uint32_t* __restrict__ b_tbl, const uint32_t
   if (i < n) ed_verify_check_body(i, b_tbl, as, rs, ss, ks, out_ok, err);
 }
 
-// The fixed-point table of B, d * 2^(16 j) * B (16 levels x 2^15 points x 96 B, 48 MiB): built by the first
-// per-signature verify after nmsm_init, freed by nmsm_shutdown.
-static int ensure_ed25519_b_table(Context& X) {
-  if (X.ed25519_b_table) return NMSM_OK;
-  uint32_t b_xy[16];
-  for (int k = 0; k < 8; k++) {
-    b_xy[k] = Ed25519Consts::GX(k);
-    b_xy[8 + k] = Ed25519Consts::GY(k);
-  }
-  int levels = 0;
-  return Engine<CurveEd25519>::build_point_table((const uint8_t*)b_xy, &X.ed25519_b_table, &levels);
-}
-
+// The check kernel walks the fixed-point table of B in Context::ed25519_b_table (16 levels x 2^15 points x 96 B,
+// 48 MiB).
 int ed25519_verify_each_impl(const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs, const uint64_t* msg_off,
                              uint64_t n, int flags, uint8_t* out_ok) {
   Context& X = g_ctx;
-  Slot& C = X.slot[0];
-  if (n == 0) return NMSM_OK;
-  if (n >= (1ull << 31)) return fail(NMSM_ERR_ARG, "n must be < 2^31");
   if (int r = check_offsets(msg_off, "msg_off", n)) return r;
-  if (int r = ensure_ed25519_b_table(X)) return r;
+  if (int r = ensure_g_table<CurveEd25519, Ed25519Consts>(&X.ed25519_b_table)) return r;
   const uint64_t msg_bytes = msg_off[n];
-  auto al = [](uint64_t x) { return (x + 255) & ~255ull; };
-  const uint64_t o_sig = 0, o_pk = o_sig + al(64 * n), o_msg = o_pk + al(32 * n), o_mo = o_msg + al(msg_bytes + 16),
-                 o_a = o_mo + al(8 * (n + 1)), o_r = o_a + al(64 * n), o_s = o_r + al(64 * n), o_k = o_s + al(32 * n),
-                 o_ok = o_k + al(32 * n), o_misc = o_ok + al(n), total = o_misc + 256;
+  const uint64_t o_sig = 0, o_pk = o_sig + al256(64 * n), o_msg = o_pk + al256(32 * n),
+                 o_mo = o_msg + al256(msg_bytes + 16), o_a = o_mo + al256(8 * (n + 1)), o_r = o_a + al256(64 * n),
+                 o_s = o_r + al256(64 * n), o_k = o_s + al256(32 * n), o_ok = o_k + al256(32 * n),
+                 o_misc = o_ok + al256(n), total = o_misc + 256;
   CK(X.ed_scratch.ensure(total));
   uint8_t* base = (uint8_t*)X.ed_scratch.p;
-  cudaStream_t st = C.stream;
+  cudaStream_t st = X.slot[0].stream;
   if (int r = h2d_any(base + o_sig, sigs, 64 * n, st)) return r;
   if (int r = h2d_any(base + o_pk, pks, 32 * n, st)) return r;
-  if (msg_bytes)
-    if (int r = h2d_any(base + o_msg, msgs, msg_bytes, st)) return r;
+  if (int r = h2d_any(base + o_msg, msgs, msg_bytes, st)) return r;
   if (int r = h2d_any(base + o_mo, msg_off, 8 * (n + 1), st)) return r;
   uint32_t *d_a = (uint32_t*)(base + o_a), *d_r = (uint32_t*)(base + o_r), *d_s = (uint32_t*)(base + o_s),
            *d_k = (uint32_t*)(base + o_k);
   uint8_t* d_ok = base + o_ok;
   unsigned int* d_err = (unsigned int*)(base + o_misc);
-  CK(cudaMemsetAsync(d_err, 0xff, 8, st));
-  EV(0);
-  k_ed_verify_prepare<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, base + o_sig, base + o_pk, base + o_msg,
-                                                    (const uint64_t*)(base + o_mo), flags, d_a, d_r, d_s, d_k, d_ok);
-  EV(1);
-  k_ed_verify_check<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, X.ed25519_b_table, d_a, d_r, d_s, d_k, d_ok, d_err);
-  EV(2);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out_ok, d_ok, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  record_verify_timing(X, C);
-  return NMSM_OK;
+  return verify_launch(
+      d_err,
+      [&] {
+        k_ed_verify_prepare<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, base + o_sig, base + o_pk, base + o_msg,
+                                                          (const uint64_t*)(base + o_mo), flags, d_a, d_r, d_s, d_k,
+                                                          d_ok);
+      },
+      [&] {
+        k_ed_verify_check<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, X.ed25519_b_table, d_a, d_r, d_s, d_k, d_ok,
+                                                        d_err);
+      },
+      d_ok, out_ok, n);
 }
 
 }  // namespace nmsm

@@ -1,8 +1,9 @@
 // P-256 (secp256r1) ECDSA batch verification (ecdsa_verify.cuh on CurveP256): the same two kernels as secp256k1's
 // k_ecdsa_prepare / k_ecdsa_check, over the a = -3 group law.  P-256 is not an MSM curve id: this unit instantiates
-// only the verification kernels, the host driver of ecdsa_nist.cuh and, through Engine<CurveP256>::build_point_table,
-// the three kernels that build the fixed-point table of G (k_prepare, k_table_base, k_table_level).
-#include "ecdsa_nist.cuh"
+// only the verification kernels, the host driver of ecdsa_driver.cuh and, through
+// Engine<CurveP256>::build_point_table, the three kernels that build the fixed-point table of G (k_prepare,
+// k_table_base, k_table_level).
+#include "ecdsa_driver.cuh"
 
 namespace nmsm {
 
@@ -36,8 +37,8 @@ k_p256_ecdsa_check(uint32_t n, const uint32_t* __restrict__ g_tbl, const uint32_
 // The fixed-point table of G: 17 levels of 2^15 points (36 MB) in Context::p256_g_table.
 int p256_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off, const uint8_t* msgs,
                            const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok) {
-  return nist_ecdsa_verify_batch<CurveP256, P256Consts>(k_p256_ecdsa_prepare, k_p256_ecdsa_check, &g_ctx.p256_g_table,
-                                                        sigs, pks, pk_off, msgs, msg_off, n, flags, out_ok);
+  return ecdsa_verify_batch<CurveP256, P256Consts>(k_p256_ecdsa_prepare, k_p256_ecdsa_check, &g_ctx.p256_g_table, sigs,
+                                                   pks, pk_off, msgs, msg_off, n, flags, out_ok);
 }
 
 }  // namespace nmsm

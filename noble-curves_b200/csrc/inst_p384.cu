@@ -1,8 +1,8 @@
 // P-384 (secp384r1) ECDSA batch verification (ecdsa_verify.cuh on CurveP384): P-256's two kernels at 12 limbs, with
 // SHA-384 as the prehash.  P-384 is not an MSM curve id: this unit instantiates only the verification kernels, the
-// host driver of ecdsa_nist.cuh and, through Engine<CurveP384>::build_point_table, the three kernels that build the
+// host driver of ecdsa_driver.cuh and, through Engine<CurveP384>::build_point_table, the three kernels that build the
 // fixed-point table of G (k_prepare, k_table_base, k_table_level).
-#include "ecdsa_nist.cuh"
+#include "ecdsa_driver.cuh"
 
 namespace nmsm {
 
@@ -37,8 +37,8 @@ k_p384_ecdsa_check(uint32_t n, const uint32_t* __restrict__ g_tbl, const uint32_
 // The fixed-point table of G: 25 levels of 2^15 points of 96 B (79 MB) in Context::p384_g_table.
 int p384_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off, const uint8_t* msgs,
                            const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok) {
-  return nist_ecdsa_verify_batch<CurveP384, P384Consts>(k_p384_ecdsa_prepare, k_p384_ecdsa_check, &g_ctx.p384_g_table,
-                                                        sigs, pks, pk_off, msgs, msg_off, n, flags, out_ok);
+  return ecdsa_verify_batch<CurveP384, P384Consts>(k_p384_ecdsa_prepare, k_p384_ecdsa_check, &g_ctx.p384_g_table, sigs,
+                                                   pks, pk_off, msgs, msg_off, n, flags, out_ok);
 }
 
 }  // namespace nmsm

@@ -2,7 +2,7 @@
 // (SURVEY §8 f5, ecdsa_verify.cuh), BIP340 Schnorr batch verification (f6, schnorr_verify.cuh) and ECDSA public-key
 // recovery / Ethereum ecrecover (f9, recover.cuh).
 #include "engine.cuh"
-#include "ecdsa_verify.cuh"
+#include "ecdsa_driver.cuh"
 #include "recover.cuh"
 #include "schnorr_verify.cuh"
 
@@ -87,98 +87,45 @@ k_recover_check(uint32_t n, const uint32_t* __restrict__ g_tbl, const uint32_t* 
   if (i < n) recover_finish<LAYOUT>(i, q_ok, acc, zi, out, ok);
 }
 
-// The fixed-point table of G that ECDSA and Schnorr verification share: d * 2^(16 j) * G, the table table_mul_body
-// walks.  Built by the first verify after nmsm_init, freed by nmsm_shutdown.
-static int ensure_secp256k1_g_table(Context& X) {
-  if (X.secp256k1_g_table) return NMSM_OK;
-  static const uint32_t g_xy[16] = {0x16f81798u, 0x59f2815bu, 0x2dce28d9u, 0x029bfcdbu, 0xce870b07u, 0x55a06295u,
-                                    0xf9dcbbacu, 0x79be667eu, 0xfb10d4b8u, 0x9c47d08fu, 0xa6855419u, 0xfd17b448u,
-                                    0x0e1108a8u, 0x5da4fbfcu, 0x26a3c465u, 0x483ada77u};
-  int levels = 0;
-  return Engine<CurveSecp256k1>::build_point_table((const uint8_t*)g_xy, &X.secp256k1_g_table, &levels);
-}
-
+// ECDSA, Schnorr verification and recovery share the fixed-point table of G in Context::secp256k1_g_table
 int secp256k1_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint64_t* pk_off, const uint8_t* msgs,
                                 const uint64_t* msg_off, uint64_t n, int flags, uint8_t* out_ok) {
-  Context& X = g_ctx;
-  Slot& C = X.slot[0];
-  if (n == 0) return NMSM_OK;
-  if (n >= (1ull << 31)) return fail(NMSM_ERR_ARG, "n must be < 2^31");
-  if (int r = check_offsets(pk_off, "pk_off", n)) return r;
-  if (int r = check_offsets(msg_off, "msg_off", n)) return r;
-  if (int r = ensure_secp256k1_g_table(X)) return r;
-  const uint64_t pk_bytes = pk_off[n], msg_bytes = msg_off[n];
-  auto al = [](uint64_t x) { return (x + 255) & ~255ull; };
-  const uint64_t o_sig = 0, o_pk = o_sig + al(64 * n), o_pko = o_pk + al(pk_bytes + 16), o_msg = o_pko + al(8 * (n + 1)),
-                 o_mo = o_msg + al(msg_bytes + 16), o_q = o_mo + al(8 * (n + 1)), o_u1 = o_q + al(64 * n),
-                 o_u2 = o_u1 + al(32 * n), o_r = o_u2 + al(32 * n), o_ok = o_r + al(32 * n), o_misc = o_ok + al(n),
-                 total = o_misc + 256;
-  CK(X.ed_scratch.ensure(total));
-  uint8_t* base = (uint8_t*)X.ed_scratch.p;
-  cudaStream_t st = C.stream;
-  if (int r = h2d_any(base + o_sig, sigs, 64 * n, st)) return r;
-  if (pk_bytes)
-    if (int r = h2d_any(base + o_pk, pks, pk_bytes, st)) return r;
-  if (int r = h2d_any(base + o_pko, pk_off, 8 * (n + 1), st)) return r;
-  if (msg_bytes)
-    if (int r = h2d_any(base + o_msg, msgs, msg_bytes, st)) return r;
-  if (int r = h2d_any(base + o_mo, msg_off, 8 * (n + 1), st)) return r;
-  uint32_t *d_q = (uint32_t*)(base + o_q), *d_u1 = (uint32_t*)(base + o_u1), *d_u2 = (uint32_t*)(base + o_u2),
-           *d_r = (uint32_t*)(base + o_r);
-  uint8_t* d_ok = base + o_ok;
-  unsigned int* d_err = (unsigned int*)(base + o_misc);
-  CK(cudaMemsetAsync(d_err, 0xff, 8, st));
-  EV(0);
-  k_ecdsa_prepare<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, base + o_sig, base + o_pk, (const uint64_t*)(base + o_pko),
-                                                base + o_msg, (const uint64_t*)(base + o_mo), flags, d_q, d_u1, d_u2, d_r,
-                                                d_ok);
-  EV(1);
-  k_ecdsa_check<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, X.secp256k1_g_table, d_q, d_u1, d_u2, d_r, d_ok, d_err);
-  EV(2);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out_ok, d_ok, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  record_verify_timing(X, C);
-  return NMSM_OK;
+  return ecdsa_verify_batch<CurveSecp256k1, Secp256k1Consts>(k_ecdsa_prepare, k_ecdsa_check, &g_ctx.secp256k1_g_table,
+                                                             sigs, pks, pk_off, msgs, msg_off, n, flags, out_ok);
 }
 
 int secp256k1_schnorr_verify_batch_impl(const uint8_t* sigs, const uint8_t* pks, const uint8_t* msgs,
                                         const uint64_t* msg_off, uint64_t n, uint8_t* out_ok) {
   Context& X = g_ctx;
-  Slot& C = X.slot[0];
-  if (n == 0) return NMSM_OK;
-  if (n >= (1ull << 31)) return fail(NMSM_ERR_ARG, "n must be < 2^31");
   if (int r = check_offsets(msg_off, "msg_off", n)) return r;
-  if (int r = ensure_secp256k1_g_table(X)) return r;
+  if (int r = ensure_g_table<CurveSecp256k1, Secp256k1Consts>(&X.secp256k1_g_table)) return r;
   const uint64_t msg_bytes = msg_off[n];
-  auto al = [](uint64_t x) { return (x + 255) & ~255ull; };
-  const uint64_t o_sig = 0, o_pk = o_sig + al(64 * n), o_msg = o_pk + al(32 * n), o_mo = o_msg + al(msg_bytes + 16),
-                 o_p = o_mo + al(8 * (n + 1)), o_s = o_p + al(64 * n), o_u = o_s + al(32 * n), o_r = o_u + al(32 * n),
-                 o_ok = o_r + al(32 * n), o_misc = o_ok + al(n), total = o_misc + 256;
+  const uint64_t o_sig = 0, o_pk = o_sig + al256(64 * n), o_msg = o_pk + al256(32 * n),
+                 o_mo = o_msg + al256(msg_bytes + 16), o_p = o_mo + al256(8 * (n + 1)), o_s = o_p + al256(64 * n),
+                 o_u = o_s + al256(32 * n), o_r = o_u + al256(32 * n), o_ok = o_r + al256(32 * n),
+                 o_misc = o_ok + al256(n), total = o_misc + 256;
   CK(X.ed_scratch.ensure(total));
   uint8_t* base = (uint8_t*)X.ed_scratch.p;
-  cudaStream_t st = C.stream;
+  cudaStream_t st = X.slot[0].stream;
   if (int r = h2d_any(base + o_sig, sigs, 64 * n, st)) return r;
   if (int r = h2d_any(base + o_pk, pks, 32 * n, st)) return r;
-  if (msg_bytes)
-    if (int r = h2d_any(base + o_msg, msgs, msg_bytes, st)) return r;
+  if (int r = h2d_any(base + o_msg, msgs, msg_bytes, st)) return r;
   if (int r = h2d_any(base + o_mo, msg_off, 8 * (n + 1), st)) return r;
   uint32_t *d_p = (uint32_t*)(base + o_p), *d_s = (uint32_t*)(base + o_s), *d_u = (uint32_t*)(base + o_u),
            *d_r = (uint32_t*)(base + o_r);
   uint8_t* d_ok = base + o_ok;
   unsigned int* d_err = (unsigned int*)(base + o_misc);
-  CK(cudaMemsetAsync(d_err, 0xff, 8, st));
-  EV(0);
-  k_schnorr_prepare<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, base + o_sig, base + o_pk, base + o_msg,
-                                                  (const uint64_t*)(base + o_mo), d_p, d_s, d_u, d_r, d_ok);
-  EV(1);
-  k_schnorr_check<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, X.secp256k1_g_table, d_p, d_s, d_u, d_r, d_ok, d_err);
-  EV(2);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out_ok, d_ok, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  record_verify_timing(X, C);
-  return NMSM_OK;
+  return verify_launch(
+      d_err,
+      [&] {
+        k_schnorr_prepare<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, base + o_sig, base + o_pk, base + o_msg,
+                                                        (const uint64_t*)(base + o_mo), d_p, d_s, d_u, d_r, d_ok);
+      },
+      [&] {
+        k_schnorr_check<<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, X.secp256k1_g_table, d_p, d_s, d_u, d_r, d_ok,
+                                                      d_err);
+      },
+      d_ok, out_ok, n);
 }
 
 // The host side of both recovery entry points: in = n x 65 B (RECOVER_SIG65, with msgs / msg_off) or n x 128 B
@@ -189,44 +136,37 @@ static int recover_batch_impl(const uint8_t* in, const uint8_t* msgs, const uint
   constexpr bool SIG65 = LAYOUT == RECOVER_SIG65;
   constexpr uint64_t IN_BYTES = SIG65 ? 65 : 128, OUT_WORDS = SIG65 ? 16 : 8;
   Context& X = g_ctx;
-  Slot& C = X.slot[0];
-  if (n == 0) return NMSM_OK;
-  if (n >= (1ull << 31)) return fail(NMSM_ERR_ARG, "n must be < 2^31");
   if (SIG65)
     if (int r = check_offsets(msg_off, "msg_off", n)) return r;
-  if (int r = ensure_secp256k1_g_table(X)) return r;
+  if (int r = ensure_g_table<CurveSecp256k1, Secp256k1Consts>(&X.secp256k1_g_table)) return r;
   const uint64_t msg_bytes = SIG65 ? msg_off[n] : 0;
-  auto al = [](uint64_t x) { return (x + 255) & ~255ull; };
-  const uint64_t o_in = 0, o_msg = o_in + al(IN_BYTES * n), o_mo = o_msg + al(msg_bytes + 16),
-                 o_r = o_mo + al(SIG65 ? 8 * (n + 1) : 0), o_u1 = o_r + al(64 * n), o_u2 = o_u1 + al(32 * n),
-                 o_out = o_u2 + al(32 * n), o_ok = o_out + al(4 * OUT_WORDS * n), o_misc = o_ok + al(n),
+  const uint64_t o_in = 0, o_msg = o_in + al256(IN_BYTES * n), o_mo = o_msg + al256(msg_bytes + 16),
+                 o_r = o_mo + al256(SIG65 ? 8 * (n + 1) : 0), o_u1 = o_r + al256(64 * n), o_u2 = o_u1 + al256(32 * n),
+                 o_out = o_u2 + al256(32 * n), o_ok = o_out + al256(4 * OUT_WORDS * n), o_misc = o_ok + al256(n),
                  total = o_misc + 256;
   CK(X.ed_scratch.ensure(total));
   uint8_t* base = (uint8_t*)X.ed_scratch.p;
-  cudaStream_t st = C.stream;
+  cudaStream_t st = X.slot[0].stream;
   if (int r = h2d_any(base + o_in, in, IN_BYTES * n, st)) return r;
-  if (msg_bytes)
-    if (int r = h2d_any(base + o_msg, msgs, msg_bytes, st)) return r;
+  if (int r = h2d_any(base + o_msg, msgs, msg_bytes, st)) return r;
   if (SIG65)
     if (int r = h2d_any(base + o_mo, msg_off, 8 * (n + 1), st)) return r;
   uint32_t *d_r = (uint32_t*)(base + o_r), *d_u1 = (uint32_t*)(base + o_u1), *d_u2 = (uint32_t*)(base + o_u2),
            *d_out = (uint32_t*)(base + o_out);
   uint8_t* d_ok = base + o_ok;
   unsigned int* d_err = (unsigned int*)(base + o_misc);
-  CK(cudaMemsetAsync(d_err, 0xff, 8, st));
-  EV(0);
-  k_recover_prepare<LAYOUT><<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, base + o_in, base + o_msg,
-                                                          (const uint64_t*)(base + o_mo), flags, d_r, d_u1, d_u2, d_ok);
-  EV(1);
-  k_recover_check<LAYOUT><<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, X.secp256k1_g_table, d_r, d_u1, d_u2, d_ok, d_out,
-                                                        d_err);
-  EV(2);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out, d_out, 4 * OUT_WORDS * n, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(out_ok, d_ok, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  record_verify_timing(X, C);
-  return NMSM_OK;
+  return verify_launch(
+      d_err,
+      [&] {
+        k_recover_prepare<LAYOUT><<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, base + o_in, base + o_msg,
+                                                                (const uint64_t*)(base + o_mo), flags, d_r, d_u1, d_u2,
+                                                                d_ok);
+      },
+      [&] {
+        k_recover_check<LAYOUT><<<cdiv(n, 128), 128, 0, st>>>((uint32_t)n, X.secp256k1_g_table, d_r, d_u1, d_u2, d_ok,
+                                                              d_out, d_err);
+      },
+      d_ok, out_ok, n, d_out, out, 4 * OUT_WORDS * n);
 }
 
 int secp256k1_recover_batch_impl(const uint8_t* sigs65, const uint8_t* msgs, const uint64_t* msg_off, uint64_t n,

@@ -85,8 +85,6 @@ int pairing_checks_run(Context& X, Slot& C, const PairingKernels& K, uint64_t n_
   return NMSM_OK;
 }
 
-uint64_t al256(uint64_t x) { return (x + 255) & ~255ull; }
-
 // bytes of the Miller workspace: PAIRING_CHUNK values and the two carry slots
 template <class P>
 constexpr uint64_t pairing_workspace_bytes() {

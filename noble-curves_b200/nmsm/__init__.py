@@ -446,6 +446,10 @@ def _pack_scalars(scalars: Sequence[int]) -> bytes:
     return b"".join(s.to_bytes(32, "little") for s in scalars)
 
 
+def _cp(b: bytes):
+    return ctypes.cast(ctypes.c_char_p(b or b"\0"), ctypes.c_void_p)
+
+
 def _raise_mapped(e: NmsmError):
     # the C ABI already carries the reference's message text for point/scalar errors
     raise ValueError(str(e)) from e
@@ -863,8 +867,7 @@ def ed25519_verify_batch_packed(sigs: bytes, pks: bytes, msgs: bytes, msg_off: b
     lib = _lib.load()
     ok = ctypes.c_int(0)
     bad = ctypes.c_longlong(-1)
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    rc = lib.nmsm_ed25519_verify_batch(cp(sigs), cp(pks), cp(msgs or b"\0"), cp(msg_off), n, cp(z), ctypes.byref(ok),
+    rc = lib.nmsm_ed25519_verify_batch(_cp(sigs), _cp(pks), _cp(msgs or b"\0"), _cp(msg_off), n, _cp(z), ctypes.byref(ok),
                                        ctypes.byref(bad))
     try:
         _lib.check(rc)
@@ -908,8 +911,7 @@ def ed25519_verify_each_packed(sigs: bytes, pks: bytes, msgs: bytes, msg_off: by
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    rc = lib.nmsm_ed25519_verify_each(cp(sigs or b"\0"), cp(pks or b"\0"), cp(msgs or b"\0"), cp(msg_off), n,
+    rc = lib.nmsm_ed25519_verify_each(_cp(sigs or b"\0"), _cp(pks or b"\0"), _cp(msgs or b"\0"), _cp(msg_off), n,
                                       0 if zip215 else ED25519_VERIFY_STRICT, out)
     try:
         _lib.check(rc)
@@ -952,37 +954,47 @@ def _check_ecdsa_args(signatures, messages, public_keys, sig_len: int = 64):
             raise ValueError('"compact signature" expected Uint8Array of length %d, got length=%d' % (sig_len, len(s)))
 
 
+def _ecdsa_verify_batch(fn: str, sig_len: int, signatures, messages, public_keys, prehash: bool,
+                        lowS: bool) -> List[bool]:
+    """the list form of the ECDSA entry point fn (nmsm_<curve>_verify_batch) with sig_len-byte signatures"""
+    _check_ecdsa_args(signatures, messages, public_keys, sig_len)
+    flags = (ECDSA_PREHASH if prehash else 0) | (ECDSA_LOW_S if lowS else 0)
+    out = _ecdsa_verify_batch_packed(fn, sig_len, b"".join(bytes(s) for s in signatures),
+                                     b"".join(bytes(p) for p in public_keys), _pack_offsets(public_keys),
+                                     b"".join(bytes(m) for m in messages), _pack_offsets(messages), len(signatures),
+                                     flags)
+    return [b == 1 for b in out]
+
+
+def _ecdsa_verify_batch_packed(fn: str, sig_len: int, sigs: bytes, pks: bytes, pk_off: bytes, msgs: bytes,
+                               msg_off: bytes, n: int, flags: int) -> bytes:
+    """the C call of the ECDSA entry point fn on caller-packed arrays"""
+    if len(sigs) != sig_len * n or len(pk_off) != 8 * (n + 1) or len(msg_off) != 8 * (n + 1):
+        raise ValueError("packed arrays do not match n")
+    _lib.ensure_init()
+    lib = _lib.load()
+    out = ctypes.create_string_buffer(max(n, 1))
+    rc = getattr(lib, fn)(_cp(sigs), _cp(pks), _cp(pk_off), _cp(msgs), _cp(msg_off), n, flags, out)
+    try:
+        _lib.check(rc)
+    except NmsmError as e:
+        _raise_mapped(e)
+    return out.raw[:n]
+
+
 def ecdsa_verify_batch(signatures, messages, public_keys, prehash: bool = True, lowS: bool = True) -> List[bool]:
     """Batch form of secp256k1.verify(sig, msg, publicKey, {prehash, lowS}) with format 'compact' (noble-curves
     weierstrass.ts ecdsa().verify): one verdict per signature.  Raises where the reference throws before its `try`
     (non-bytes arguments, a signature that is not 64 bytes) and for lists of different lengths; everything else
     (r, s out of range, high s, an undecodable key, a raw message over 8192 bytes, R = O) is a False verdict."""
-    _check_ecdsa_args(signatures, messages, public_keys)
-    n = len(signatures)
-    flags = (ECDSA_PREHASH if prehash else 0) | (ECDSA_LOW_S if lowS else 0)
-    out = ecdsa_verify_batch_packed(b"".join(bytes(s) for s in signatures), b"".join(bytes(p) for p in public_keys),
-                                    _pack_offsets(public_keys), b"".join(bytes(m) for m in messages),
-                                    _pack_offsets(messages), n, flags)
-    return [b == 1 for b in out]
+    return _ecdsa_verify_batch("nmsm_secp256k1_verify_batch", 64, signatures, messages, public_keys, prehash, lowS)
 
 
 def ecdsa_verify_batch_packed(sigs: bytes, pks: bytes, pk_off: bytes, msgs: bytes, msg_off: bytes, n: int,
                               flags: int = ECDSA_PREHASH | ECDSA_LOW_S) -> bytes:
     """The C-ABI call itself (nmsm_secp256k1_verify_batch) on caller-packed arrays: n*64 signature bytes, the
     concatenated keys and messages with n+1 little-endian u64 offsets each.  Returns n verdict bytes (1 = valid)."""
-    if len(sigs) != 64 * n or len(pk_off) != 8 * (n + 1) or len(msg_off) != 8 * (n + 1):
-        raise ValueError("packed arrays do not match n")
-    _lib.ensure_init()
-    lib = _lib.load()
-    out = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    rc = lib.nmsm_secp256k1_verify_batch(cp(sigs or b"\0"), cp(pks or b"\0"), cp(pk_off), cp(msgs or b"\0"),
-                                         cp(msg_off), n, flags, out)
-    try:
-        _lib.check(rc)
-    except NmsmError as e:
-        _raise_mapped(e)
-    return out.raw[:n]
+    return _ecdsa_verify_batch_packed("nmsm_secp256k1_verify_batch", 64, sigs, pks, pk_off, msgs, msg_off, n, flags)
 
 
 def _secp256k1_verify(signature, message, publicKey, prehash: bool = True, lowS: bool = True,
@@ -1001,32 +1013,14 @@ def p256_ecdsa_verify_batch(signatures, messages, public_keys, prehash: bool = T
     weierstrass.ts ecdsa().verify): one verdict per signature.  The defaults are noble's for p256 (lowS false, as
     OpenSSL).  Raises as ecdsa_verify_batch; everything else (r, s out of range, high s under lowS, an undecodable key,
     a raw message over 8192 bytes, R = O) is a False verdict."""
-    _check_ecdsa_args(signatures, messages, public_keys)
-    flags = (ECDSA_PREHASH if prehash else 0) | (ECDSA_LOW_S if lowS else 0)
-    out = p256_ecdsa_verify_batch_packed(b"".join(bytes(s) for s in signatures),
-                                         b"".join(bytes(p) for p in public_keys), _pack_offsets(public_keys),
-                                         b"".join(bytes(m) for m in messages), _pack_offsets(messages),
-                                         len(signatures), flags)
-    return [b == 1 for b in out]
+    return _ecdsa_verify_batch("nmsm_p256_verify_batch", 64, signatures, messages, public_keys, prehash, lowS)
 
 
 def p256_ecdsa_verify_batch_packed(sigs: bytes, pks: bytes, pk_off: bytes, msgs: bytes, msg_off: bytes, n: int,
                                    flags: int = ECDSA_PREHASH) -> bytes:
     """The C-ABI call itself (nmsm_p256_verify_batch) on caller-packed arrays, laid out as for
     ecdsa_verify_batch_packed.  Returns n verdict bytes (1 = valid)."""
-    if len(sigs) != 64 * n or len(pk_off) != 8 * (n + 1) or len(msg_off) != 8 * (n + 1):
-        raise ValueError("packed arrays do not match n")
-    _lib.ensure_init()
-    lib = _lib.load()
-    out = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    rc = lib.nmsm_p256_verify_batch(cp(sigs or b"\0"), cp(pks or b"\0"), cp(pk_off), cp(msgs or b"\0"), cp(msg_off), n,
-                                    flags, out)
-    try:
-        _lib.check(rc)
-    except NmsmError as e:
-        _raise_mapped(e)
-    return out.raw[:n]
+    return _ecdsa_verify_batch_packed("nmsm_p256_verify_batch", 64, sigs, pks, pk_off, msgs, msg_off, n, flags)
 
 
 def _p256_verify(signature, message, publicKey, prehash: bool = True, lowS: bool = False,
@@ -1091,32 +1085,14 @@ def p384_ecdsa_verify_batch(signatures, messages, public_keys, prehash: bool = T
     or 97-byte uncompressed SEC1, and prehash hashes with SHA-384.  The defaults are noble's for p384 (lowS false, as
     OpenSSL).  Raises as p256_ecdsa_verify_batch; everything else (r, s out of range, high s under lowS, an undecodable
     key, a raw message over 8192 bytes, R = O) is a False verdict."""
-    _check_ecdsa_args(signatures, messages, public_keys, sig_len=96)
-    flags = (ECDSA_PREHASH if prehash else 0) | (ECDSA_LOW_S if lowS else 0)
-    out = p384_ecdsa_verify_batch_packed(b"".join(bytes(s) for s in signatures),
-                                         b"".join(bytes(p) for p in public_keys), _pack_offsets(public_keys),
-                                         b"".join(bytes(m) for m in messages), _pack_offsets(messages),
-                                         len(signatures), flags)
-    return [b == 1 for b in out]
+    return _ecdsa_verify_batch("nmsm_p384_verify_batch", 96, signatures, messages, public_keys, prehash, lowS)
 
 
 def p384_ecdsa_verify_batch_packed(sigs: bytes, pks: bytes, pk_off: bytes, msgs: bytes, msg_off: bytes, n: int,
                                    flags: int = ECDSA_PREHASH) -> bytes:
     """The C-ABI call itself (nmsm_p384_verify_batch) on caller-packed arrays: n*96 signature bytes, the concatenated
     keys and messages with n+1 little-endian u64 offsets each.  Returns n verdict bytes (1 = valid)."""
-    if len(sigs) != 96 * n or len(pk_off) != 8 * (n + 1) or len(msg_off) != 8 * (n + 1):
-        raise ValueError("packed arrays do not match n")
-    _lib.ensure_init()
-    lib = _lib.load()
-    out = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    rc = lib.nmsm_p384_verify_batch(cp(sigs or b"\0"), cp(pks or b"\0"), cp(pk_off), cp(msgs or b"\0"), cp(msg_off), n,
-                                    flags, out)
-    try:
-        _lib.check(rc)
-    except NmsmError as e:
-        _raise_mapped(e)
-    return out.raw[:n]
+    return _ecdsa_verify_batch_packed("nmsm_p384_verify_batch", 96, sigs, pks, pk_off, msgs, msg_off, n, flags)
 
 
 def _p384_verify(signature, message, publicKey, prehash: bool = True, lowS: bool = False,
@@ -1161,8 +1137,7 @@ def schnorr_verify_batch_packed(sigs: bytes, pks: bytes, msgs: bytes, msg_off: b
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    rc = lib.nmsm_secp256k1_schnorr_verify_batch(cp(sigs or b"\0"), cp(pks or b"\0"), cp(msgs or b"\0"), cp(msg_off), n,
+    rc = lib.nmsm_secp256k1_schnorr_verify_batch(_cp(sigs or b"\0"), _cp(pks or b"\0"), _cp(msgs or b"\0"), _cp(msg_off), n,
                                                  out)
     try:
         _lib.check(rc)
@@ -1218,8 +1193,7 @@ def ecdsa_recover_batch_packed(sigs65: bytes, msgs: bytes, msg_off: bytes, n: in
     lib = _lib.load()
     xy = ctypes.create_string_buffer(max(64 * n, 1))
     ok = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    rc = lib.nmsm_secp256k1_recover_batch(cp(sigs65 or b"\0"), cp(msgs or b"\0"), cp(msg_off), n, flags, xy, ok)
+    rc = lib.nmsm_secp256k1_recover_batch(_cp(sigs65 or b"\0"), _cp(msgs or b"\0"), _cp(msg_off), n, flags, xy, ok)
     try:
         _lib.check(rc)
     except NmsmError as e:
@@ -1265,8 +1239,7 @@ def eth_ecrecover_batch_packed(inputs128: bytes, n: int):
     lib = _lib.load()
     words = ctypes.create_string_buffer(max(32 * n, 1))
     ok = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    rc = lib.nmsm_secp256k1_ecrecover_batch(cp(inputs128 or b"\0"), n, words, ok)
+    rc = lib.nmsm_secp256k1_ecrecover_batch(_cp(inputs128 or b"\0"), n, words, ok)
     try:
         _lib.check(rc)
     except NmsmError as e:
@@ -1312,8 +1285,7 @@ def _pairing_check_call(fn: str, g1_bytes: int, g1_xy: bytes, g2_xy: bytes, pair
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(n_checks, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    _lib.check(getattr(lib, fn)(cp(g1_xy or b"\0"), cp(g2_xy or b"\0"), cp(pair_off), n_checks, out))
+    _lib.check(getattr(lib, fn)(_cp(g1_xy or b"\0"), _cp(g2_xy or b"\0"), _cp(pair_off), n_checks, out))
     return out.raw[:n_checks]
 
 
@@ -1393,8 +1365,7 @@ def bls_verify_batch_packed(sigs96: bytes, pks48: bytes, msg_pts: bytes, n: int)
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    _lib.check(lib.nmsm_bls12_381_verify_batch(cp(sigs96 or b"\0"), cp(pks48 or b"\0"), cp(msg_pts or b"\0"), n, out))
+    _lib.check(lib.nmsm_bls12_381_verify_batch(_cp(sigs96 or b"\0"), _cp(pks48 or b"\0"), _cp(msg_pts or b"\0"), n, out))
     return out.raw[:n]
 
 
@@ -1452,8 +1423,7 @@ def bls_hash_to_g2_batch_packed(msgs: bytes, msg_off: bytes, n: int, dst: bytes)
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(192 * n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    _lib.check(lib.nmsm_bls12_381_hash_to_g2_batch(cp(msgs or b"\0"), cp(msg_off), n, cp(dst or b"\0"), len(dst), out))
+    _lib.check(lib.nmsm_bls12_381_hash_to_g2_batch(_cp(msgs or b"\0"), _cp(msg_off), n, _cp(dst or b"\0"), len(dst), out))
     return out.raw[:192 * n]
 
 
@@ -1499,9 +1469,8 @@ def bls_verify_messages_batch_packed(sigs96: bytes, pks48: bytes, msgs: bytes, m
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    _lib.check(lib.nmsm_bls12_381_verify_msg_batch(cp(sigs96 or b"\0"), cp(pks48 or b"\0"), cp(msgs or b"\0"),
-                                                   cp(msg_off), n, cp(dst or b"\0"), len(dst), out))
+    _lib.check(lib.nmsm_bls12_381_verify_msg_batch(_cp(sigs96 or b"\0"), _cp(pks48 or b"\0"), _cp(msgs or b"\0"),
+                                                   _cp(msg_off), n, _cp(dst or b"\0"), len(dst), out))
     return out.raw[:n]
 
 
@@ -1605,10 +1574,9 @@ def bls_aggregate_verify_batch_packed(sigs96: bytes, group_off: bytes, msgs: byt
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(n_checks, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    _lib.check(lib.nmsm_bls12_381_aggregate_verify_batch(cp(sigs96 or b"\0"), cp(group_off), n_checks,
-                                                         cp(msgs or b"\0"), cp(msg_off), cp(keys_xy or b"\0"),
-                                                         cp(key_off), cp(dst or b"\0"), len(dst), out))
+    _lib.check(lib.nmsm_bls12_381_aggregate_verify_batch(_cp(sigs96 or b"\0"), _cp(group_off), n_checks,
+                                                         _cp(msgs or b"\0"), _cp(msg_off), _cp(keys_xy or b"\0"),
+                                                         _cp(key_off), _cp(dst or b"\0"), len(dst), out))
     return out.raw[:n_checks]
 
 
@@ -1678,8 +1646,7 @@ def bls_hash_to_g1_batch_packed(msgs: bytes, msg_off: bytes, n: int, dst: bytes)
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(96 * n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    _lib.check(lib.nmsm_bls12_381_hash_to_g1_batch(cp(msgs or b"\0"), cp(msg_off), n, cp(dst or b"\0"), len(dst), out))
+    _lib.check(lib.nmsm_bls12_381_hash_to_g1_batch(_cp(msgs or b"\0"), _cp(msg_off), n, _cp(dst or b"\0"), len(dst), out))
     return out.raw[:96 * n]
 
 
@@ -1753,8 +1720,7 @@ def bls_short_verify_batch_packed(sigs48: bytes, pks96: bytes, msg_pts: bytes, n
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    _lib.check(lib.nmsm_bls12_381_short_verify_batch(cp(sigs48 or b"\0"), cp(pks96 or b"\0"), cp(msg_pts or b"\0"), n,
+    _lib.check(lib.nmsm_bls12_381_short_verify_batch(_cp(sigs48 or b"\0"), _cp(pks96 or b"\0"), _cp(msg_pts or b"\0"), n,
                                                      out))
     return out.raw[:n]
 
@@ -1786,9 +1752,8 @@ def bls_short_verify_messages_batch_packed(sigs48: bytes, pks96: bytes, msgs: by
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    _lib.check(lib.nmsm_bls12_381_short_verify_msg_batch(cp(sigs48 or b"\0"), cp(pks96 or b"\0"), cp(msgs or b"\0"),
-                                                         cp(msg_off), n, cp(dst or b"\0"), len(dst), out))
+    _lib.check(lib.nmsm_bls12_381_short_verify_msg_batch(_cp(sigs48 or b"\0"), _cp(pks96 or b"\0"), _cp(msgs or b"\0"),
+                                                         _cp(msg_off), n, _cp(dst or b"\0"), len(dst), out))
     return out.raw[:n]
 
 
@@ -1871,11 +1836,10 @@ def kzg_verify_proof_batch_packed(commitments48: bytes, zs32: bytes, ys32: bytes
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    vh = cp(versioned_hashes32) if versioned_hashes32 is not None else None
-    _lib.check(lib.nmsm_bls12_381_kzg_verify_proof_batch(cp(commitments48 or b"\0"), cp(zs32 or b"\0"),
-                                                         cp(ys32 or b"\0"), cp(proofs48 or b"\0"), vh, n,
-                                                         cp(setup_g2_96), out))
+    vh = _cp(versioned_hashes32) if versioned_hashes32 is not None else None
+    _lib.check(lib.nmsm_bls12_381_kzg_verify_proof_batch(_cp(commitments48 or b"\0"), _cp(zs32 or b"\0"),
+                                                         _cp(ys32 or b"\0"), _cp(proofs48 or b"\0"), vh, n,
+                                                         _cp(setup_g2_96), out))
     return out.raw[:n]
 
 
@@ -1904,9 +1868,8 @@ def kzg_verify_blob_proof_batch_packed(blobs: bytes, commitments48: bytes, proof
     _lib.ensure_init()
     lib = _lib.load()
     out = ctypes.create_string_buffer(max(n, 1))
-    cp = lambda b: ctypes.cast(ctypes.c_char_p(b), ctypes.c_void_p)  # noqa: E731
-    _lib.check(lib.nmsm_bls12_381_kzg_verify_blob_batch(cp(blobs or b"\0"), cp(commitments48 or b"\0"),
-                                                        cp(proofs48 or b"\0"), n, cp(setup_g2_96), out))
+    _lib.check(lib.nmsm_bls12_381_kzg_verify_blob_batch(_cp(blobs or b"\0"), _cp(commitments48 or b"\0"),
+                                                        _cp(proofs48 or b"\0"), n, _cp(setup_g2_96), out))
     return out.raw[:n]
 
 
@@ -1968,7 +1931,7 @@ class KzgSetup:
         self._lib = _lib.load()
         h = ctypes.c_uint64(0)
         try:
-            _lib.check(self._lib.nmsm_bls12_381_kzg_setup_create(_kzg_cp(buf), ctypes.byref(h)))
+            _lib.check(self._lib.nmsm_bls12_381_kzg_setup_create(_cp(buf), ctypes.byref(h)))
         except NmsmError as e:
             _raise_mapped(e)
         self.handle = h.value
@@ -1978,7 +1941,7 @@ class KzgSetup:
         bytes); raises NmsmError on an error."""
         _kzg_check_packed(blobs, n)
         out, ok = ctypes.create_string_buffer(max(48 * n, 1)), ctypes.create_string_buffer(max(n, 1))
-        _lib.check(self._lib.nmsm_bls12_381_kzg_commit_batch(self.handle, _kzg_cp(blobs), n, out, ok))
+        _lib.check(self._lib.nmsm_bls12_381_kzg_commit_batch(self.handle, _cp(blobs), n, out, ok))
         return out.raw[:48 * n], ok.raw[:n]
 
     def compute_kzg_proof_batch_packed(self, blobs: bytes, zs32: bytes, n: int):
@@ -1987,7 +1950,7 @@ class KzgSetup:
         _kzg_check_packed(blobs, n, zs32, 32)
         out, ys = ctypes.create_string_buffer(max(48 * n, 1)), ctypes.create_string_buffer(max(32 * n, 1))
         ok = ctypes.create_string_buffer(max(n, 1))
-        _lib.check(self._lib.nmsm_bls12_381_kzg_compute_proof_batch(self.handle, _kzg_cp(blobs), _kzg_cp(zs32), n, out,
+        _lib.check(self._lib.nmsm_bls12_381_kzg_compute_proof_batch(self.handle, _cp(blobs), _cp(zs32), n, out,
                                                                     ys, ok))
         return out.raw[:48 * n], ys.raw[:32 * n], ok.raw[:n]
 
@@ -1996,8 +1959,8 @@ class KzgSetup:
         bytes -> (n*48 proof bytes, n ok bytes); raises NmsmError on an error."""
         _kzg_check_packed(blobs, n, commitments48, 48)
         out, ok = ctypes.create_string_buffer(max(48 * n, 1)), ctypes.create_string_buffer(max(n, 1))
-        _lib.check(self._lib.nmsm_bls12_381_kzg_compute_blob_proof_batch(self.handle, _kzg_cp(blobs),
-                                                                         _kzg_cp(commitments48), n, out, ok))
+        _lib.check(self._lib.nmsm_bls12_381_kzg_compute_blob_proof_batch(self.handle, _cp(blobs),
+                                                                         _cp(commitments48), n, out, ok))
         return out.raw[:48 * n], ok.raw[:n]
 
     def blob_to_kzg_commitment_batch(self, blobs) -> List[Optional[bytes]]:
@@ -2041,10 +2004,6 @@ class KzgSetup:
             self.close()
         except Exception:
             pass
-
-
-def _kzg_cp(b: bytes):
-    return ctypes.cast(ctypes.c_char_p(b or b"\0"), ctypes.c_void_p)
 
 
 def _kzg_check_packed(blobs: bytes, n: int, other: bytes = b"", width: int = 0):
